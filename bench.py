@@ -1,24 +1,31 @@
 #!/usr/bin/env python
-"""bench.py -- samples/s of the DLRM fwd+bwd+optimizer hot path on N B200s (contract in the task statement).
+"""bench.py -- samples/s of the DLRM fwd+bwd+optimizer hot path on N H100s.
 One "step" = one pass of the hot path (index exchange, forward, loss, backward, fused row-wise-Adagrad embedding
 update, dense update) over one synthetic batch.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload cfg3|cfg2|cfg1]
+                    [--dump-outputs DIR]
 
 Workloads (BASELINE.json configs)
   cfg3 (default, every N): MLPerf-DLRM synthetic -- the config the headline metric is quoted on: 26 tables of the
-        Criteo-Terabyte sizes (204 M rows x dim 128 = 104.5 GB fp32, fits one B200), multi-hot bags of fixed length
-        L_k (214 lookups per sample), bot 13-512-256-128, top 479-1024-1024-512-256-1, batch 8192 PER GPU (global
-        65536 at 8 GPUs: weak scaling), fwd+bwd+RWSAdagrad.  Tables are placed by dlrm_b200/placement.py
-        (cost-balanced, the L=100 / L=27 tables row-split over all ranks).
+        Criteo-Terabyte sizes with every table capped at 20 M rows, as the reference's --max-ind-range caps them
+        (104.2 M rows x dim 128 = 53.3 GB fp32, 55 GB with the per-row optimizer words: fits one 80 GB H100),
+        multi-hot bags of fixed length L_k (214 lookups per sample), bot 13-512-256-128, top
+        479-1024-1024-512-256-1, batch 8192 PER GPU (global 65536 at 8 GPUs: weak scaling), fwd+bwd+RWSAdagrad.
+        Tables are placed by dlrm_b200/placement.py (cost-balanced, the L=100 / L=27 tables row-split over all
+        ranks).
   cfg2: 26 x 1e6 x 128 tables, random bags of <= 10 indices, bot 13-512-256-128, top 479-1024-512-256-1, batch
         2048 per GPU (round 1's headline);  cfg1: cfg2's model, forward only.
 
 Every N (1 included) runs the same sharded engine (one process per GPU; N = 1 is a 1-rank group).  Timing:
-a ring of >= 8 distinct pre-generated batches (their touched rows exceed the 126 MB L2 many times over: "inputs
+a ring of >= 8 distinct pre-generated batches (their touched rows exceed the 50 MB L2 many times over: "inputs
 larger than L2"); CUDA events on the launching stream; max over ranks; nvidia-smi clocks sampled during the
 timed region.  `value`: the packed batches already sit in HBM.  `e2e`: packed pinned host batches -> one H2D
 copy per step (copy stream, double-buffered) -> step -> loss D2H.
+
+--dump-outputs DIR writes what the last device-resident timed step computed (rank 0) as DIR/<name>.npy: the loss,
+the predictions, the dense parameters after the update and a fixed, seeded sample of embedding rows and their
+accumulators.  Inputs and initial parameters are fixed by seeds, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -36,6 +43,8 @@ import torch
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
+CFG3_MAX_ROWS = 20_000_000       # per-table row cap of cfg3 (--max-ind-range): 26 tables fit one 80 GB GPU
+DUMP_ROWS = 32768                 # embedding rows in the --dump-outputs sample (16 MB)
 CFG2 = dict(m_spa=128, rows=[1_000_000] * 26, ln_bot=[13, 512, 256, 128], top_tail=[1024, 512, 256, 1], B=2048,
             lmax=10, hot=None)
 
@@ -44,12 +53,12 @@ def workload(name, world=1):
     from dlrm_b200 import mlperf as M
 
     if name == "cfg4":
-        # BASELINE.json configs[4]: one giant row-split table (2e9 rows x 128 = 1 TB fp32 at 8 GPUs: 2.5e8 rows =
-        # 128 GB per GPU, scaled with N) + 25 tables of 1e6 rows, random bags, batch 8192 per GPU (65536 at 8)
-        return dict(m_spa=128, rows=[250_000_000 * world] + [1_000_000] * 25, ln_bot=[13, 512, 256, 128],
+        # one giant row-split table (8e7 rows x 128 = 42 GB per GPU with the per-row optimizer words, scaled with
+        # N: 6.4e8 rows at 8 GPUs) + 25 tables of 1e6 rows, random bags, batch 8192 per GPU (65536 at 8)
+        return dict(m_spa=128, rows=[80_000_000 * world] + [1_000_000] * 25, ln_bot=[13, 512, 256, 128],
                     top_tail=[1024, 512, 256, 1], B=8192, lmax=10, hot=None)
     if name == "cfg3":
-        return dict(m_spa=M.DIM, rows=list(M.TABLE_ROWS), ln_bot=list(M.LN_BOT), top_tail=list(M.TOP_TAIL), B=8192,
+        return dict(m_spa=M.DIM, rows=[min(r, CFG3_MAX_ROWS) for r in M.TABLE_ROWS], ln_bot=list(M.LN_BOT), top_tail=list(M.TOP_TAIL), B=8192,
                     lmax=None, hot=list(M.MULTI_HOT))
     return dict(CFG2)
 
@@ -208,10 +217,11 @@ def metric_name(train):
 
 
 def config_dict(args, W, n):
-    desc = {"cfg3": "cfg3: MLPerf-DLRM synthetic, 26 Criteo-Terabyte-sized tables (204.18 M rows x 128, 104.5 GB fp32), "
+    desc = {"cfg3": "cfg3: MLPerf-DLRM synthetic, 26 Criteo-Terabyte-sized tables capped at 20 M rows (104.18 M rows x 128, "
+                    "53.3 GB fp32), "
                     "multi-hot L_k sum 214, bot 13-512-256-128, top 479-1024-1024-512-256-1, batch 8192/GPU, "
                     "fwd+bwd+RWSAdagrad",
-            "cfg4": "cfg4: ONE row-split table of 2.5e8 x N rows x 128 (1 TB fp32 at N=8) + 25 x 1e6 x 128 tables, bot "
+            "cfg4": "cfg4: ONE row-split table of 8e7 x N rows x 128 (41 GB fp32 per GPU) + 25 x 1e6 x 128 tables, bot "
                     "13-512-256-128, top 479-1024-512-256-1, batch 8192/GPU, random data Lmax=10, fwd+bwd+RWSAdagrad",
             "cfg2": "cfg2: 26x1e6x128 tables, bot 13-512-256-128, top 479-1024-512-256-1, batch 2048/GPU, random data "
                     "Lmax=10, fwd+bwd+RWSAdagrad",
@@ -239,7 +249,10 @@ def parity_check(de_cls, dev, gemm):
     from dlrm_b200 import placement as P, sharding as S
     from dlrm_b200.engine import sparse_from_reference
 
-    z = np.load(os.path.join(ROOT, "tests", "golden", "cfg0.npz"))
+    from oracle import dlrm_numpy as O
+
+    z = dict(np.load(os.path.join(ROOT, "tests", "golden", "cfg0.npz")))
+    z.update(np.load(os.path.join(ROOT, "tests", "golden", "cfg0_rwsadagrad.npz")))
     rank, world = dist.get_rank(), dist.get_world_size()
     D, ln_emb = int(z["m_spa"]), [int(v) for v in z["ln_emb"]]
     ln_bot, ln_top = [int(v) for v in z["ln_bot"]], [int(v) for v in z["ln_top"]]
@@ -248,9 +261,7 @@ def parity_check(de_cls, dev, gemm):
     pl = P.plan(ln_emb, [5.0] * T, world, force_split=[0] if world <= 2 else [])
     de = de_cls(D, ln_emb, ln_bot, ln_top, local_batch=B, device=dev, gemm=gemm, exchange="p2p", placement=pl,
                 loss=str(z["loss"]), semantics="single_process")   # the golden is a single-process run of the batch
-    params = dict(emb=[z["emb%d" % k] for k in range(T)],
-                  bot=[(z["botW%d" % i], z["botb%d" % i]) for i in range(len(ln_bot) - 1)],
-                  top=[(z["topW%d" % i], z["topb%d" % i]) for i in range(len(ln_top) - 1)], v_W_l=None)
+    params = O.random_params(np.random.default_rng(int(z["seed"])), D, ln_emb, ln_bot, ln_top)   # the golden's weights
     de.eng.load_params(S.slice_params(params, pl, rank))
     lr = float(z["rwsadagrad_lr"])
     nsteps = int(z["nsteps"])
@@ -477,10 +488,12 @@ def ours(args, W):
     n0 = de.eng.n_launch
     ev0.record()
     for r in range(args.steps):
-        resident_step(args.warmup + r)
+        out = resident_step(args.warmup + r)
     ev1.record()
     sync_all()
     t1 = time.time()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, de.eng, out, B, train)
     launches = de.eng.n_launch - n0
     ms = torch.tensor([ev0.elapsed_time(ev1) / args.steps], device=dev)
     if world > 1:
@@ -549,7 +562,7 @@ def ours(args, W):
             "metric": metric_name(train), "value": Bg / (ms * 1e-3), "unit": "samples/s", "n_gpus": world,
             "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None,
-            "dtype": {"simt": "fp32", "tc": "fp32 (bf16x3 split on tcgen05, fp32 accumulate)", "tc_bf16": "bf16"}[args.gemm],
+            "dtype": {"simt": "fp32", "tc": "fp32 (bf16x3 split on wgmma, fp32 accumulate)", "tc_bf16": "bf16"}[args.gemm],
             "data": "synthetic", "config": config_dict(args, W, world),
             "roofline": None, "roofline_update": None, "cpu_baseline": None,
             "e2e": {"value": Bg / (ms2 * 1e-3), "unit": "samples/s", "h2d_bytes_per_step": int(h2d / args.steps),
@@ -586,8 +599,9 @@ def ours(args, W):
                 peaks = json.load(fh)
         except Exception:
             pass
-        hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s"
+        hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+        peak_src = ("measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks
+                    else "H100 SXM data sheet 3350 GB/s (not a measured peak)")
         try:
             roof, roof_upd = measure_rooflines(de, stages, load_dev, pre, args, W, cost, hbm_peak, peak_src, train)
             prog.extra.update(roofline=roof, roofline_update=roof_upd)
@@ -636,10 +650,8 @@ def ours(args, W):
                   "marks": [[n, round(float(np.mean(acc[n])), 1)] for n in order]}
         if rank == 0:       # AFTER the bench line (a separate stderr line + file): the bench line stays the one stdout line
             print("phases " + json.dumps(phases), file=sys.stderr, flush=True)
-            out = args.phases_out or (os.path.join(ROOT, "gpurun_out", "phases_%s_n%d.json" % (args.workload, world))
-                                      if os.path.isdir(os.path.join(ROOT, "gpurun_out")) else None)
-            if out:
-                with open(out, "w") as fh:
+            if args.phases_out:
+                with open(args.phases_out, "w") as fh:
                     json.dump(phases, fh)
     prog.stage("teardown")
     try:
@@ -654,21 +666,18 @@ def ours(args, W):
         os._exit(0)
 
 
-def ncu_traffic(kernel, path="profiles/r2_ncu_full_cfg3_gather_update.csv"):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel` from the committed ncu --set full capture
-    (cfg3, batch 8192, 1 GPU; tools/gpu_r2_15.sh), in bytes; None when the file is not there."""
-    import csv
-
-    mult = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    try:
-        with open(os.path.join(ROOT, path)) as fh:
-            rows = list(csv.reader(fh))
-        h, units = rows[0], rows[1]
-        ir, iw, ik = h.index("dram__bytes_read.sum"), h.index("dram__bytes_write.sum"), h.index("Kernel Name")
-        v = [float(r[ir]) * mult[units[ir]] + float(r[iw]) * mult[units[iw]] for r in rows[2:] if kernel in r[ik]]
-        return float(np.mean(v)) if v else None
-    except Exception:
-        return None
+def dump_outputs(path, eng, out, B, train):
+    """The arrays the last timed step computed, as float32 / float64 .npy files under `path` (< 64 MB in all)."""
+    os.makedirs(path, exist_ok=True)
+    arrays = {"p": out} if not train else {"loss": out.view(-1), "p": eng.top_act[-1][:B], "dense_params": eng.dense}
+    if train:
+        g = torch.Generator().manual_seed(0)
+        idx = torch.randint(0, eng.total_rows, (DUMP_ROWS,), generator=g).sort().values.to(eng.tables.device)
+        arrays.update(emb_rows=eng.tables[idx, :eng.D], emb_accumulator=eng.momentum[idx],
+                      emb_row_index=idx.double())
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy()
+        np.save(os.path.join(path, name + ".npy"), a if a.dtype == np.float64 else a.astype(np.float32))
 
 
 def measure_rooflines(de, stages, load_dev, pre, args, W, cost, hbm_peak, peak_src, train):
@@ -718,11 +727,7 @@ def measure_rooflines(de, stages, load_dev, pre, args, W, cost, hbm_peak, peak_s
     by = nnz * D * 4 + scanned * idx_b + T * B * idx_b + T * B * D * 4  # SURVEY 8(d): rows + indices + offsets + pooled out
     ach = by / tg / 1e9
     roof = {"kernel": "emb_fwd_vec_kernel (multi-table EmbeddingBag gather, forward)", "bound": "hbm", "achieved": ach,
-            "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak,
-            "traffic": ncu_traffic("emb_fwd_vec_kernel") if (args.workload == "cfg3" and de.world == 1) else None,
-            "traffic_source": "profiles/r2_ncu_full_cfg3_gather_update.csv: dram read + write bytes per launch of the "
-                              "training gather (ncu --set full, same workload; the forward-only gather differs by the "
-                              "14 MB list-entry stream)", "peak_source": peak_src,
+            "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak, "peak_source": peak_src,
             "avg_launch_us": tg * 1e6, "algorithmic_bytes_per_launch": by,
             "how": "CUDA events around each gather launch on the launching stream, median of %d over the batch ring" % n}
     roof_upd = None
@@ -749,7 +754,6 @@ def measure_rooflines(de, stages, load_dev, pre, args, W, cost, hbm_peak, peak_s
         achu = by_u / tu / 1e9
         roof_upd = {"kernel": "emb_update_kernel (+ emb_small_*: coalesce + row-wise Adagrad, in place)", "bound": "hbm",
                     "achieved": achu, "peak": hbm_peak, "unit": "GB/s", "frac": achu / hbm_peak,
-                    "traffic": ncu_traffic("emb_update_lean_kernel") if (args.workload == "cfg3" and de.world == 1) else None,
                     "avg_launch_us": tu * 1e6, "algorithmic_bytes_per_launch": by_u,
                     "train_gather_plus_link_us": t_gl * 1e6,
                     "train_gather": {"achieved": by / t_gl / 1e9, "frac": by / t_gl / 1e9 / hbm_peak},
@@ -775,7 +779,13 @@ def main():
     ap.add_argument("--no-check", action="store_true", help="skip the pre-run parity check against the live-reference golden")
     ap.add_argument("--cpu-budget", type=float, default=15.0)
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the arrays the last timed step computed to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs writes what the GPU path computed; it needs --impl ours")
     args.warmup = max(args.warmup, 3)
     W = workload(args.workload, max(int(os.environ.get("WORLD_SIZE", "1")), 1))
     if args.impl == "reference":

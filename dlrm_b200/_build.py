@@ -1,5 +1,5 @@
-"""Build libdlrm_b200.so in-tree with nvcc for sm_100a (no JIT cache: the .so must travel
-with the repo snapshot to the GPU box)."""
+"""Build libdlrm_b200.so in-tree with nvcc for sm_90a (H100).  The library is built ahead of time by
+`__graft_entry__.build()` and loaded from the tree, so a run needs no compiler and no JIT cache."""
 import glob
 import hashlib
 import os
@@ -13,7 +13,7 @@ LIB = os.path.join(LIBDIR, "libdlrm_b200.so")
 STAMP = os.path.join(LIBDIR, "libdlrm_b200.stamp")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared", "--use_fast_math=false",
 ]
 NVCC_FLAGS = [f for f in NVCC_FLAGS if not f.startswith("--use_fast_math")]
@@ -24,9 +24,9 @@ def sources():
 
 
 def _digest():
-    """Hash of the sources' CONTENTS and names -- not of their absolute paths: the library built in the build
-    container must count as fresh in any copy of the tree (the GPU box runs a snapshot under a scratch path, and a
-    path-dependent digest made every first process there rebuild the library, all ranks of a torchrun at once)."""
+    """Hash of the sources' CONTENTS and names -- not of their absolute paths: a library built once must count as
+    fresh in any copy of the tree (a path-dependent digest would make every first process of a copied tree rebuild
+    the library, all ranks of a torchrun at once)."""
     h = hashlib.sha256()
     for f in sources() + sorted(glob.glob(os.path.join(CSRC, "*.cuh"))) + [
             os.path.join(os.path.dirname(HERE), "include", "dlrm_b200.h")]:

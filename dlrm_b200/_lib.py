@@ -191,7 +191,7 @@ def device_info(device=0):
 
 
 class GemmTcPlan:
-    """RAII wrapper of a tcgen05 GEMM plan (TMA descriptors + launch geometry)."""
+    """RAII wrapper of a wgmma GEMM plan (TMA descriptors + launch geometry)."""
 
     def __init__(self, **kw):
         d = GemmTcDesc()

@@ -1,5 +1,5 @@
 """`python dlrm_s_pytorch.py <flags>` -- the reference's command line (dlrm_s_pytorch.py:902-1021) driving
-the B200 engine, so that `bench/dlrm_s_benchmark.sh` runs unmodified from this repo's root.
+the H100 engine, so that `bench/dlrm_s_benchmark.sh` runs unmodified from this repo's root.
 
 Every flag of the reference is accepted with the same default.  Flags that select subsystems outside
 the hot path (datasets, QR/MD embeddings, quantisation, ONNX, mlperf logging, ...) exit with the

@@ -79,8 +79,8 @@ extern "C" int dlrm_b200_device_info(int device, int* sm_count, int* cc_major, i
   if (sm_count) *sm_count = prop.multiProcessorCount;
   if (cc_major) *cc_major = prop.major;
   if (cc_minor) *cc_minor = prop.minor;
-  if (prop.major < 10)
-    return dlrm::set_error("device %d is sm_%d%d; libdlrm_b200 is built for sm_100a only", device,
+  if (prop.major != 9 || prop.minor != 0)
+    return dlrm::set_error("device %d is sm_%d%d; libdlrm_b200 is built for sm_90a (H100) only", device,
                            prop.major, prop.minor);
   return 0;
 }

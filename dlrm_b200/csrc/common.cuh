@@ -1,4 +1,4 @@
-// Shared helpers for libdlrm_b200.so (sm_100a only).
+// Shared helpers for libdlrm_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -22,7 +22,7 @@ enum Tunable {
   TUNE_EMB_BLOCK = 2,           // threads per CTA in the gather
   TUNE_UPD_BLOCK = 3,
   TUNE_GEMM_SPLITK = 4,
-  TUNE_GEMM_SMEM_KB = 5,        // operand-ring budget per GEMM CTA at plan creation (0 = 200 KB = 1 CTA/SM)
+  TUNE_GEMM_SMEM_KB = 5,        // operand-ring budget per GEMM CTA at plan creation (0 = 200 KB, the deepest ring)
   TUNE_HEAD_ROWS = 6,           // samples per CTA in the fused head (16 or 32; 0 = default)
   TUNE_INTERACT_BWD_COLS = 7,   // 1 = one column per thread (first kernel), else float2 columns
   TUNE_PDL = 8,                 // programmatic dependent launch on the dense chain: 0/1 = on, 2 = off

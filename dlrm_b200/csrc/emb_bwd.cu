@@ -13,7 +13,8 @@
 //            Depends on the indices only -> can overlap the forward pass.
 //   update : one warp per bag.  Occurrence `pos` owns its row iff head[row] == pos + 1 (the
 //            last arrival).  The owner walks the list, sorts the members by position when there
-//            are <= 32 (deterministic sum in ascending position == grad.coalesce() order), adds
+//            are <= 32 (deterministic sum in ascending position == grad.coalesce() order; a longer list
+//            takes the order-independent fixed-point sum of list_sum_exact), adds
 //            their dY rows, applies the optimizer to the 512-byte weight row in registers and
 //            resets head[row] = 0.  Non-owners do nothing.  Rows without duplicates (the common
 //            case at 1e6-row tables) never touch link[] beyond their own entry and reuse the
@@ -36,6 +37,94 @@ __device__ __forceinline__ void list_walk_guard(unsigned& chunks, unsigned long 
       __trap();
     }
   }
+}
+
+// Sum of the dY rows of a row's occurrence list longer than 32 (the owner `self_bag` first, then the list from
+// `nxt`).  The list is built by atomicExch, so its order changes from run to run; summing it in list order would
+// make the update -- and every later step -- differ between runs.  Instead every value is converted to 64-bit fixed
+// point with a per-column scale taken from the column's largest magnitude (a max, independent of order), the
+// integers are added exactly and the sum is rounded to fp32 once: the result depends only on the set of members.
+// The conversion truncates at 2^-62 x n of the column's largest |value|, far below one fp32 ulp of the sum.
+// Called by a whole warp.  The walk gathers 32 members per chunk into the lanes (one dependent link load each);
+// the bags of the first LS_KEEP chunks stay in registers, so the second pass over them only reloads dY rows.
+// load(bag, t) fills t[0..N) with this lane's columns of the dY row of `bag` (0 for columns outside the row).
+constexpr int LS_KEEP = 4;
+
+struct ListWalk {
+  const int2* link;
+  int cur, self_bag;
+  bool first;
+  unsigned chunks;
+  unsigned long long t0;
+  // next <= 32 members into the lanes (member i of the chunk -> lane i's `bag`); returns their number
+  __device__ __forceinline__ int chunk(int lane, int& bag) {
+    int cnt = 0;
+    while (cnt < 32 && (first || cur != 0)) {
+      int b;
+      if (first) { b = self_bag; first = false; }
+      else { const int2 e = link[cur - 1]; b = e.y; cur = e.x; }
+      if (lane == cnt) bag = b;
+      ++cnt;
+    }
+    list_walk_guard(chunks, t0);
+    return cnt;
+  }
+  __device__ __forceinline__ bool done() const { return !first && cur == 0; }
+};
+
+template <int N, class Load>
+__device__ __forceinline__ void list_sum_exact(const int2* link, int nxt, int self_bag, const Load& load, float (&out)[N]) {
+  const int lane = threadIdx.x & 31;
+  float mx[N];
+#pragma unroll
+  for (int j = 0; j < N; ++j) mx[j] = 0.f;
+  int keep[LS_KEEP];
+  int cnt_keep[LS_KEEP];
+  ListWalk w{link, nxt, self_bag, true, 0u, 0ull};
+  ListWalk resume = w;
+  int n = 0;
+  for (int c = 0; !w.done(); ++c) {                    // pass 1: column maxima
+    int bag = 0;
+    const int cnt = w.chunk(lane, bag);
+    if (c < LS_KEEP) { keep[c] = bag; cnt_keep[c] = cnt; resume = w; }
+    for (int q = 0; q < cnt; ++q) {
+      float t[N];
+      load(__shfl_sync(0xffffffffu, bag, q), t);
+#pragma unroll
+      for (int j = 0; j < N; ++j) mx[j] = fmaxf(mx[j], fabsf(t[j]));
+    }
+    n += cnt;
+  }
+  const int L = 32 - __clz(n);                          // n < 2^L
+  double sc[N];
+  long long s[N];
+  float f[N];                                          // plain sum: only to carry an inf / nan through
+#pragma unroll
+  for (int j = 0; j < N; ++j) {
+    int E;
+    frexpf(mx[j], &E);                                  // |value| < 2^E  ->  |sum| x 2^k < 2^62
+    sc[j] = ldexp(1.0, 62 - L - E);
+    s[j] = 0;
+    f[j] = 0.f;
+  }
+  auto add_chunk = [&](int bag, int cnt) {
+    for (int q = 0; q < cnt; ++q) {
+      float t[N];
+      load(__shfl_sync(0xffffffffu, bag, q), t);
+#pragma unroll
+      for (int j = 0; j < N; ++j) { s[j] += (long long)((double)t[j] * sc[j]); f[j] += t[j]; }
+    }
+  };
+#pragma unroll
+  for (int c = 0; c < LS_KEEP; ++c)                    // pass 2: the kept chunks, then the rest of the list
+    if (c * 32 < n) add_chunk(keep[c], cnt_keep[c]);
+  while (!resume.done()) {
+    int bag = 0;
+    const int cnt = resume.chunk(lane, bag);
+    add_chunk(bag, cnt);
+  }
+#pragma unroll
+  for (int j = 0; j < N; ++j) out[j] = isfinite(f[j]) ? (float)((double)s[j] / sc[j]) : f[j];
 }
 
 struct EmbBwdTable {
@@ -231,6 +320,30 @@ __global__ void __launch_bounds__(256) emb_link_suspects_kernel(const __grid_con
 // reads index / link / head with coalesced + gathered loads, and processes the rows it owns with
 // up to PF weight rows AND their dY rows in flight.  The bag of an occurrence comes from link[],
 // so the offsets are not needed (packed format reads only the per-table bounds).
+// Out of line: the long-list sum must not take registers from the update kernel's hot path.
+template <int NV, int W>
+__device__ __noinline__ void dup_sum_long(const EmbBwdParams& P, int nxt, int self_bag, long long dyk_off,
+                                          const bool (&col_ok)[NV], Pack<W> (&g)[NV]) {
+  const int lane = threadIdx.x & 31;
+  auto load = [&](int bag, float (&t)[NV * W]) {
+#pragma unroll
+    for (int v = 0; v < NV; ++v) {
+      Pack<W> p;
+#pragma unroll
+      for (int e = 0; e < W; ++e) p.x[e] = 0.f;
+      if (col_ok[v]) p = ld_pack<W>(dy_row(P, bag) + dyk_off + lane * W + v * 32 * W);
+#pragma unroll
+      for (int e = 0; e < W; ++e) t[v * W + e] = p.x[e];
+    }
+  };
+  float acc[NV * W];
+  list_sum_exact<NV * W>(P.link, nxt, self_bag, load, acc);
+#pragma unroll
+  for (int v = 0; v < NV; ++v)
+#pragma unroll
+    for (int e = 0; e < W; ++e) g[v].x[e] = acc[v * W + e];
+}
+
 template <int W, int NV, typename idx_t>
 __global__ void __launch_bounds__(256, NV == 1 ? 3 : 1) emb_update_kernel(const __grid_constant__ EmbBwdParams P,
                                                                           int num_tables, long long total_hint) {
@@ -310,24 +423,23 @@ __global__ void __launch_bounds__(256, NV == 1 ? 3 : 1) emb_update_kernel(const 
         for (int v = 0; v < NV; ++v) { w[v] = wpf[u][v]; g[v] = gpf[u][v]; }
         const float m_old = mpf[u];
         if (nxt != 0) {
-          // duplicates: gather members (self first), in chunks of 32, sorted by position
+          // duplicates: up to 32 members (self first) are summed in ascending position (== grad.coalesce());
+          // a longer list takes the order-independent sum
 #pragma unroll
           for (int v = 0; v < NV; ++v)
 #pragma unroll
             for (int e = 0; e < W; ++e) g[v].x[e] = 0.f;
+          const int nxt0 = nxt;
           int cnt = 1;
           int mpos = (lane == 0) ? (int)(base + src) : 0x7fffffff;
           int mbag = self_bag;
-          unsigned walk_chunks = 0;
-          unsigned long long walk_t0 = 0;
-          while (true) {
-            if (nxt != 0 && cnt < 32) {
-              const int2 e = P.link[nxt - 1];
-              if (lane == cnt) { mpos = nxt - 1; mbag = e.y; }
-              ++cnt;
-              nxt = e.x;
-              if (nxt != 0 && cnt < 32) continue;
-            }
+          while (nxt != 0 && cnt < 32) {
+            const int2 e = P.link[nxt - 1];
+            if (lane == cnt) { mpos = nxt - 1; mbag = e.y; }
+            ++cnt;
+            nxt = e.x;
+          }
+          if (nxt == 0) {
             int rank = 0;  // positions are unique -> ranks are a permutation
             for (int i = 0; i < cnt; ++i) rank += (__shfl_sync(0xffffffffu, mpos, i) < mpos) ? 1 : 0;
             for (int q = 0; q < cnt; ++q) {
@@ -342,10 +454,8 @@ __global__ void __launch_bounds__(256, NV == 1 ? 3 : 1) emb_update_kernel(const 
                 }
               }
             }
-            if (nxt == 0) break;
-            list_walk_guard(walk_chunks, walk_t0);
-            cnt = 0;
-            mpos = 0x7fffffff;
+          } else {
+            dup_sum_long<NV, W>(P, nxt0, self_bag, dyk_off, col_ok, g);
           }
         }
         if (P.optimizer == DLRM_OPT_RWSADAGRAD) {
@@ -386,10 +496,9 @@ __global__ void __launch_bounds__(256, NV == 1 ? 3 : 1) emb_update_kernel(const 
 // ---------------------------------------------------------------------------------------------
 // Lean variant for dim <= 128 (one float4 per lane), the shape of every BASELINE config.
 //
-// The kernel above spends ~190 warp instructions per occurrence (ncu, profiles/README.md: 755 per 4): the
-// table descriptor is re-read from parameter space for every row, rows / tables / bags travel through
-// 64-bit shuffles twice, the optimizer divides per element.  At MLPerf sizes (1.75 M occurrences per step and
-// GPU) that made the update INSTRUCTION-bound at 0.19 of the HBM peak (bench r2_08).  Here
+// In the kernel above the table descriptor is re-read from parameter space for every row, rows / tables / bags
+// travel through 64-bit shuffles twice and the optimizer divides per element: at MLPerf sizes (1.75 M occurrences
+// per step and GPU) that makes the update instruction-bound instead of bound by random DRAM accesses.  Here
 //   * the per-table fields live in shared memory, a 32-position window takes its table from lane 0 unless
 //     the window straddles a table boundary;
 //   * every lane resolves ITS occurrence once into two pointers (weight row, gradient row) + the list head;
@@ -408,37 +517,44 @@ struct UpdTableS {
   long long pair_base, ld, mom_stride, hs, dy_off, row_lo, row_n;
 };
 
+__device__ __noinline__ float4 upd_sum_long(const EmbBwdParams& P, int nxt, int self_bag, long long dy_off,
+                                            bool col_ok) {
+  const int lane = threadIdx.x & 31;
+  auto load = [&](int bag, float (&t)[4]) {
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (col_ok) v = *reinterpret_cast<const float4*>(dy_row(P, bag) + dy_off + lane * 4);
+    t[0] = v.x; t[1] = v.y; t[2] = v.z; t[3] = v.w;
+  };
+  float s[4];
+  list_sum_exact<4>(P.link, nxt, self_bag, load, s);
+  return make_float4(s[0], s[1], s[2], s[3]);
+}
+
 __device__ __noinline__ float4 upd_sum_duplicates(const EmbBwdParams& P, int nxt, int self_pos, int self_bag,
                                                   long long dy_off, int lane, bool col_ok) {
-  // members of the row's list (self first), in chunks of 32, each chunk summed in ascending position
+  // up to 32 members of the row's list (self first) are summed in ascending position (== grad.coalesce());
+  // a longer list takes the order-independent sum
   float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
+  const int nxt0 = nxt;
   int cnt = 1;
   int mpos = (lane == 0) ? self_pos : 0x7fffffff;
   int mbag = self_bag;
-  unsigned walk_chunks = 0;
-  unsigned long long walk_t0 = 0;
-  while (true) {
-    if (nxt != 0 && cnt < 32) {
-      const int2 e = P.link[nxt - 1];
-      if (lane == cnt) { mpos = nxt - 1; mbag = e.y; }
-      ++cnt;
-      nxt = e.x;
-      if (nxt != 0 && cnt < 32) continue;
+  while (nxt != 0 && cnt < 32) {
+    const int2 e = P.link[nxt - 1];
+    if (lane == cnt) { mpos = nxt - 1; mbag = e.y; }
+    ++cnt;
+    nxt = e.x;
+  }
+  if (nxt != 0) return upd_sum_long(P, nxt0, self_bag, dy_off, col_ok);
+  int rank = 0;
+  for (int i = 0; i < cnt; ++i) rank += (__shfl_sync(0xffffffffu, mpos, i) < mpos) ? 1 : 0;
+  for (int q = 0; q < cnt; ++q) {
+    const unsigned who = __ballot_sync(0xffffffffu, lane < cnt && rank == q);
+    const int bag = __shfl_sync(0xffffffffu, mbag, __ffs(who) - 1);
+    if (col_ok) {
+      const float4 t = *reinterpret_cast<const float4*>(dy_row(P, bag) + dy_off + lane * 4);
+      g.x += t.x; g.y += t.y; g.z += t.z; g.w += t.w;
     }
-    int rank = 0;
-    for (int i = 0; i < cnt; ++i) rank += (__shfl_sync(0xffffffffu, mpos, i) < mpos) ? 1 : 0;
-    for (int q = 0; q < cnt; ++q) {
-      const unsigned who = __ballot_sync(0xffffffffu, lane < cnt && rank == q);
-      const int bag = __shfl_sync(0xffffffffu, mbag, __ffs(who) - 1);
-      if (col_ok) {
-        const float4 t = *reinterpret_cast<const float4*>(dy_row(P, bag) + dy_off + lane * 4);
-        g.x += t.x; g.y += t.y; g.z += t.z; g.w += t.w;
-      }
-    }
-    if (nxt == 0) break;
-    list_walk_guard(walk_chunks, walk_t0);
-    cnt = 0;
-    mpos = 0x7fffffff;
   }
   return g;
 }
@@ -757,11 +873,10 @@ static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, i
     long long gl = (total / 32 + block / 32) / (block / 32);
     if (gl > (long long)sms * 3) gl = (long long)sms * 3;
     if (gl < 1) gl = 1;
-    // TUNE_UPD_LEAN (cfg3 update, us, tools/upd_variants.py on one B200): 0/3 (default) = 2 row pairs in flight per warp,
-    // 3 CTAs/SM: 797; 5 = 3 pairs, 3 CTAs/SM: 838; 4 = 2 pairs, 3 CTAs/SM, software-pipelined windows: 848; 1 = pipelined,
-    // 3 pairs, 2 CTAs/SM: 983-1004; 6 / 7 = 4 pairs, 2 CTAs/SM, pipelined / not: 991 / 984 (2 = the general kernel).
-    // More rows in flight per warp and hiding the two leading round trips do not pay: the kernel is bound by the RATE
-    // of random accesses (list head + accumulator, row read, row write), not by the latency of any one of them.
+    // TUNE_UPD_LEAN (variants compared with tools/upd_variants.py): 0/3 (default) = 2 row pairs in flight per warp,
+    // 3 CTAs/SM; 5 = 3 pairs, 3 CTAs/SM; 4 = 2 pairs, 3 CTAs/SM, software-pipelined windows; 1 = pipelined, 3 pairs,
+    // 2 CTAs/SM; 6 / 7 = 4 pairs, 2 CTAs/SM, pipelined / not (2 = the general kernel).  The kernel is bound by the
+    // RATE of random accesses (list head + accumulator, row read, row write), not by the latency of any one of them.
     int var = (int)get_tunable(TUNE_UPD_LEAN);
     if (var == 0) var = 3;
     const int per_sm = (var == 1 || var == 6 || var == 7) ? 2 : 3;

@@ -85,9 +85,8 @@ __device__ __forceinline__ long long bag_end(const idx_t* off, long long b, long
 }
 
 // G lanes per bag, NV float4 per lane (dim = 4*G*NV when exact; columns >= dim are masked).
-// grid = (groups of S bags, table).  Measured on B200 (profiles/r1_gather_sweep_*.json): the plain grid
-// at 64 registers / 4 CTAs per SM (S=4, U=8: 32.8 us = 5.1 TB/s) beats a persistent one-wave grid at 78
-// registers / 3 CTAs per SM (34-42 us): the gather is latency-bound, resident warps matter most.
+// grid = (groups of S bags, table): a plain grid at 64 registers / 4 CTAs per SM rather than a persistent one-wave
+// grid with more registers per thread -- the gather is latency-bound, so resident warps matter most.
 template <int G, int NV, int U, typename idx_t, bool WEIGHTED, bool LINK>
 __global__ void __launch_bounds__(256, (G == 32 && NV == 1) ? 4 : 1) emb_fwd_vec_kernel(
     const __grid_constant__ EmbFwdParams P, int num_tables) {

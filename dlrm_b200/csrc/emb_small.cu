@@ -19,7 +19,7 @@
 
 namespace dlrm {
 
-constexpr int SMALL_CHUNK = 128;        // samples per accumulate CTA (512: 185 us at MLPerf batch 8192 -- 16 chunks x 8 tables cannot fill 148 SMs)
+constexpr int SMALL_CHUNK = 128;        // samples per accumulate CTA (512 would leave 16 chunks x 8 tables at MLPerf batch 8192: too few CTAs to fill the SMs)
 constexpr int SMALL_MAX_TABLES = 32;
 
 struct SmallTable {

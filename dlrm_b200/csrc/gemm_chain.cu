@@ -1,27 +1,26 @@
-// Persistent tile-dataflow tcgen05 kernel: a whole MLP chain (forward layers, or the dgrad chain with
+// Persistent tile-dataflow wgmma kernel: a whole MLP chain (forward layers, or the dgrad chain with
 // all weight-gradient GEMMs beside it) in ONE launch.
 //
-// Why: at batch 2048 every layer of the DLRM MLPs is a 32-144-tile GEMM whose math takes 1-3 us; as one
-// launch per layer each paid launch + prologue (TMEM allocation, barrier init, descriptor fetch) +
-// pipeline fill + drain, 10-30 us apiece, 17 launches per step (profiles/r1_final_launches_tc_step.csv:
-// 278 of 540 us).  Here the tiles of ALL layers of a chain are one topologically ordered task list:
+// Why: at batch 2048 every layer of the DLRM MLPs is a 32-144-tile GEMM whose math takes a few us; as one
+// launch per layer each pays launch + prologue (barrier init, descriptor fetch) + pipeline fill + drain.
+// Here the tiles of ALL layers of a chain are one topologically ordered task list:
 //
 //   * grid = one CTA per SM (or fewer); warp 0 claims the next task from a device-side queue
-//     (atomicAdd, claimed one task ahead so the round trip is hidden) and publishes it to the other
-//     warps through a 4-deep shared-memory ring guarded by mbarriers;
+//     (atomicAdd, claimed one task ahead so the round trip is hidden), publishes it to the consumer
+//     warps through a 4-deep shared-memory ring guarded by mbarriers and streams its operands;
 //   * a task whose A operand is produced inside this launch (layer l+1 reads layer l's activations;
 //     a weight-gradient GEMM reads the dgrad chain's gz) spins on per-(producer, 128-row block)
 //     completion counters (ld.acquire.gpu), then issues a async-proxy fence before its TMA loads.  Tasks
 //     are claimed in topological order and a claimed task depends only on lower-numbered tasks, which are
 //     owned by resident CTAs: no deadlock whatever the number of resident CTAs;
-//   * warp 1 issues tcgen05.mma into one of 4 TMEM accumulators (512 columns allocated once), warps 2-5
-//     run the epilogue of tile i (tcgen05.ld, activation / activation-gradient mask, fp32 and (hi,lo) bf16
-//     stores) while the MMAs of tile i+1 run; after their stores they bump the completion counter
+//   * the two consumer warpgroups run the wgmmas of tile i, stage the accumulator in shared memory and run
+//     its epilogue (activation / activation-gradient mask, fp32 and (hi,lo) bf16 stores) while the producer
+//     already streams the operands of tile i+1; after their stores they bump the completion counter
 //     (fence + named barrier + release reduction);
 //   * the last CTA to leave zeroes queue + counters, so a CUDA-graph replay needs no memset node.
 //
-// The CTA program per tile (TMA boxes, UMMA descriptors, epilogue) is the one of gemm_tc_body.cuh, so the
-// results are bit-identical to the per-layer launches.
+// The CTA program per tile (TMA boxes, smem descriptors, main loop, epilogue) is the one of
+// gemm_tc_body.cuh, so the results are bit-identical to the per-layer launches.
 #include <string.h>
 
 #include "gemm_tc_common.cuh"
@@ -29,7 +28,6 @@
 namespace dlrm {
 
 constexpr int CH_MAX_PROBLEMS = 16;
-constexpr int CH_ACC_STAGES = 4;    // 4 x 128 TMEM columns
 constexpr int CH_RING = 4;
 
 struct ChProblem {
@@ -59,17 +57,15 @@ struct ChParams {
   ChGroup grp[CH_MAX_PROBLEMS];
   int ngroups;
   int n, total, stages;
+  int max_bn;         // widest tile: size of the accumulator staging
   uint32_t stage_bytes;
   int* ctr;           // [0] task queue, [1] exit count, [2...] completion counters
   int n_ctr;
   // optional per-task timeline (globaltimer ns), 8 words per task: claim, deps ready, last TMA issued,
-  // first operands landed, last MMA issued, accumulator ready, epilogue + signal done, SM id
+  // consumers start, wgmmas retired, accumulator staged, epilogue + signal done, SM id
   unsigned long long* trace;
 };
 
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
 __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
   int v;
   asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -107,6 +103,18 @@ __device__ __forceinline__ ChTask ch_decode(const ChParams& P, int t) {
 
 constexpr int CH_EPI_WARPS = TC_EPI_WARPS;
 constexpr int CH_THREADS = TC_THREADS;
+constexpr int CH_HEAD = 512;        // barriers + task ring
+
+template <int BN>
+__device__ __forceinline__ void ch_mma_stage(const TcArgs& g, uint32_t ring, uint32_t stage_bytes, int stages,
+                                             uint32_t bar_full, uint32_t bar_empty, int kb0, int kb1, int& stage,
+                                             uint32_t& phase, float* acc, int cw, int lane) {
+  float d[BN / 2];
+  tc_mainloop<BN>(d, g, ring, stage_bytes, stages, bar_full, bar_empty, kb0, kb1, stage, phase, cw >> 2, lane);
+  // the previous task's epilogue has read the staged accumulator before it is overwritten
+  asm volatile("bar.sync 2, %0;" ::"n"(32 * CH_EPI_WARPS) : "memory");
+  tc_stage_acc<BN>(d, acc, cw, lane);
+}
 
 __global__ void __launch_bounds__(CH_THREADS, 1) gemm_chain_kernel(const __grid_constant__ ChParams P) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -114,47 +122,32 @@ __global__ void __launch_bounds__(CH_THREADS, 1) gemm_chain_kernel(const __grid_
   const int stages = P.stages;
   const uint32_t stage_bytes = P.stage_bytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)stages * stage_bytes);
-  // bars: full[stages] | empty[stages] | acc_full[4] | acc_empty[4] | task_full[4] | task_empty[4]
-  int* ring = reinterpret_cast<int*>(bars + 2 * stages + 2 * CH_ACC_STAGES + 2 * CH_RING);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(ring + CH_RING);
-  uint8_t* epi_stage = smem + (size_t)stages * stage_bytes + 512;   // barriers + ring + slot < 512 B
+  // bars: full[stages] | empty[stages] | task_full[4] | task_empty[4]
+  int* ring = reinterpret_cast<int*>(bars + 2 * stages + 2 * CH_RING);
+  float* acc = reinterpret_cast<float*>(smem + (size_t)stages * stage_bytes + CH_HEAD);
+  uint8_t* epi_stage = smem + (size_t)stages * stage_bytes + CH_HEAD + tc_acc_bytes(P.max_bn);
 
   pdl_launch_dependents();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t bar_full = smem_u32(bars);
   const uint32_t bar_empty = bar_full + 8 * stages;
-  const uint32_t bar_acc_full = bar_empty + 8 * stages;
-  const uint32_t bar_acc_empty = bar_acc_full + 8 * CH_ACC_STAGES;
-  const uint32_t bar_task_full = bar_acc_empty + 8 * CH_ACC_STAGES;
+  const uint32_t bar_task_full = bar_empty + 8 * stages;
   const uint32_t bar_task_empty = bar_task_full + 8 * CH_RING;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < stages; ++s) {
       mbar_init(bar_full + 8 * s, 1);
-      mbar_init(bar_empty + 8 * s, 1);
-    }
-    for (int s = 0; s < CH_ACC_STAGES; ++s) {
-      mbar_init(bar_acc_full + 8 * s, 1);
-      mbar_init(bar_acc_empty + 8 * s, CH_EPI_WARPS);     // lane 0 of each epilogue warp
+      mbar_init(bar_empty + 8 * s, CH_EPI_WARPS);        // one arrive per consumer warp
     }
     for (int s = 0; s < CH_RING; ++s) {
       mbar_init(bar_task_full + 8 * s, 1);
-      mbar_init(bar_task_empty + 8 * s, 1 + CH_EPI_WARPS);    // MMA warp + epilogue warps
+      mbar_init(bar_task_empty + 8 * s, CH_EPI_WARPS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"(512u)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();   // barriers and TMEM are set up; global memory is first touched below
+  pdl_wait();   // barriers are set up; global memory is first touched below
 
   if (warp == 0) {
     // ------------------------------------------------------------------ task claim + TMA producer
@@ -173,7 +166,7 @@ __global__ void __launch_bounds__(CH_THREADS, 1) gemm_chain_kernel(const __grid_
         const ChTask k = ch_decode(P, t);
         const ChProblem& Q = P.p[k.pi];
         const TcArgs& g = Q.a;
-        const uint32_t A_BYTES = TC_BM * TC_BK * 2;
+        const uint32_t A_BYTES = TC_A_BYTES;
         const uint32_t B_BYTES = (uint32_t)Q.bn * TC_BK * 2;
         const uint32_t tx = (g.x3 ? 2u : 1u) * (A_BYTES + B_BYTES);
         const int m0 = k.by * TC_BM, n0 = k.bx * Q.bn;
@@ -227,116 +220,54 @@ __global__ void __launch_bounds__(CH_THREADS, 1) gemm_chain_kernel(const __grid_
         t = tnext;
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    int stage = 0, slot = 0, as = 0;
-    uint32_t phase = 0, tph = 0, aph = 0;
+  } else if (warp >= TC_CONSUMER_WARP0) {
+    // ------------------------------------------------------------------ wgmma consumers + epilogue (warps 4..11)
+    const int cw = warp - TC_CONSUMER_WARP0;
+    const bool rec = P.trace && cw == 0 && lane == 0;
+    int stage = 0, slot = 0;
+    uint32_t phase = 0, tph = 0;
     while (true) {
       mbar_wait(bar_task_full + 8 * slot, tph);
-      const int t = ring[slot];
+      const int t = __shfl_sync(0xffffffffu, ring[slot], 0);   // warp-uniform: the wgmma paths below branch on it
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_task_empty + 8 * slot);
       if (++slot == CH_RING) { slot = 0; tph ^= 1; }
       if (t >= P.total) break;
       const ChTask k = ch_decode(P, t);
       const ChProblem& Q = P.p[k.pi];
-      const TcArgs& g = Q.a;
-      const uint32_t A_BYTES = TC_BM * TC_BK * 2;
-      const uint32_t B_BYTES = (uint32_t)Q.bn * TC_BK * 2;
-      const int kb0 = k.bz * g.kb_per_split;
-      const int kb1 = min(g.num_kb, kb0 + g.kb_per_split);
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)g.a_mn << 15) |
-                             ((uint32_t)g.b_mn << 16) | ((uint32_t)(Q.bn >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-      const uint32_t tmem_acc = tmem_base + (uint32_t)(as * 128);
-      mbar_wait(bar_acc_empty + 8 * as, aph ^ 1);     // epilogue has drained this accumulator
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      uint32_t accum = 0;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(bar_full + 8 * stage, phase);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (lane == 0) {
-          if (P.trace && kb == kb0) P.trace[(size_t)t * 8 + 3] = globaltimer_ns();
-          const uint32_t sa_hi = smem_base + stage * stage_bytes;
-          const uint32_t sa_lo = sa_hi + A_BYTES;
-          const uint32_t sb_hi = sa_hi + (g.x3 ? 2u : 1u) * A_BYTES;
-          const uint32_t sb_lo = sb_hi + B_BYTES;
-#pragma unroll
-          for (int kk = 0; kk < TC_BK / 16; ++kk) {
-            const uint32_t a_off = g.a_mn ? kk * 2048u : kk * 32u;
-            const uint32_t b_off = g.b_mn ? kk * 2048u : kk * 32u;
-            const uint32_t a_lbo = g.a_mn ? 8192u : 16u, b_lbo = g.b_mn ? 8192u : 16u;
-            const uint64_t ah = make_smem_desc(sa_hi + a_off, a_lbo, 1024);
-            const uint64_t bh = make_smem_desc(sb_hi + b_off, b_lbo, 1024);
-            if (g.x3) {
-              const uint64_t al = make_smem_desc(sa_lo + a_off, a_lbo, 1024);
-              const uint64_t bl = make_smem_desc(sb_lo + b_off, b_lbo, 1024);
-              umma_bf16(tmem_acc, al, bh, idesc, accum);
-              umma_bf16(tmem_acc, ah, bl, idesc, 1u);
-              umma_bf16(tmem_acc, ah, bh, idesc, 1u);
-            } else {
-              umma_bf16(tmem_acc, ah, bh, idesc, accum);
-            }
-            accum = 1u;
-          }
-          umma_commit(bar_empty + 8 * stage);
-          if (kb == kb1 - 1) {
-            umma_commit(bar_acc_full + 8 * as);
-            if (P.trace) P.trace[(size_t)t * 8 + 4] = globaltimer_ns();
-          }
-        }
-        __syncwarp();
-        if (++stage == stages) { stage = 0; phase ^= 1; }
-      }
-      if (++as == CH_ACC_STAGES) { as = 0; aph ^= 1; }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue (warps 2..9)
-    const int quad = warp & 3;            // TMEM lane quadrant this warp may access
-    const int half = (warp - 2) >> 2;     // which of the quadrant's two warps: even / odd 32-column chunks
-    int slot = 0, as = 0;
-    uint32_t tph = 0, aph = 0;
-    while (true) {
-      mbar_wait(bar_task_full + 8 * slot, tph);
-      const int t = ring[slot];
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_task_empty + 8 * slot);
-      if (++slot == CH_RING) { slot = 0; tph ^= 1; }
-      if (t >= P.total) break;
-      const ChTask k = ch_decode(P, t);
-      const ChProblem& Q = P.p[k.pi];
-      mbar_wait(bar_acc_full + 8 * as, aph);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (P.trace && warp == 2 && lane == 0) P.trace[(size_t)t * 8 + 5] = globaltimer_ns();
-      tc_epilogue_tile(Q.a, Q.bn, k.by * TC_BM, k.bx * Q.bn, k.bz, tmem_base + (uint32_t)(as * 128), quad, lane,
-                       epi_stage + (size_t)(warp - 2) * TC_EPI_WARP_BYTES, half, CH_EPI_WARPS / 4);
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_acc_empty + 8 * as);
+      const int kb0 = k.bz * Q.a.kb_per_split;
+      const int kb1 = min(Q.a.num_kb, kb0 + Q.a.kb_per_split);
+      if (rec) P.trace[(size_t)t * 8 + 3] = globaltimer_ns();
+      if (Q.bn == 128)
+        ch_mma_stage<128>(Q.a, smem_base, stage_bytes, stages, bar_full, bar_empty, kb0, kb1, stage, phase, acc, cw, lane);
+      else if (Q.bn == 64)
+        ch_mma_stage<64>(Q.a, smem_base, stage_bytes, stages, bar_full, bar_empty, kb0, kb1, stage, phase, acc, cw, lane);
+      else
+        ch_mma_stage<32>(Q.a, smem_base, stage_bytes, stages, bar_full, bar_empty, kb0, kb1, stage, phase, acc, cw, lane);
+      if (rec) P.trace[(size_t)t * 8 + 4] = globaltimer_ns();
+      asm volatile("bar.sync 1, %0;" ::"n"(32 * CH_EPI_WARPS) : "memory");
+      if (rec) P.trace[(size_t)t * 8 + 5] = globaltimer_ns();
+      tc_epilogue_tile(Q.a, Q.bn, k.by * TC_BM, k.bx * Q.bn, k.bz, acc, cw & 3, lane,
+                       epi_stage + (size_t)cw * TC_EPI_WARP_BYTES, cw >> 2, CH_EPI_WARPS / 4);
       if (Q.signal) {
         // grid-sync idiom: every epilogue thread has issued its stores (barrier), then ONE thread makes them
         // visible GPU-wide (cumulative fence) and publishes the tile with a release reduction
         asm volatile("bar.sync 1, %0;" ::"n"(32 * CH_EPI_WARPS) : "memory");
-        if (warp == 2 && lane == 0) {
+        if (cw == 0 && lane == 0) {
           __threadfence();
           asm volatile("fence.proxy.async;" ::: "memory");
           red_release_gpu_add(P.ctr + 2 + Q.ctr_base + k.by, 1);
         }
       }
-      if (P.trace && warp == 2 && lane == 0) {
+      if (rec) {
         unsigned smid;
         asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
         P.trace[(size_t)t * 8 + 6] = globaltimer_ns();
         P.trace[(size_t)t * 8 + 7] = smid;
       }
-      if (++as == CH_ACC_STAGES) { as = 0; aph ^= 1; }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   }
   __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-  }
   // the last CTA to leave resets queue + counters for the next launch / graph replay
   if (threadIdx.x == 0) {
     __threadfence();
@@ -367,6 +298,7 @@ extern "C" int dlrm_b200_gemm_chain_create(void* const* plans, const int* dep, c
   ChParams& P = c->P;
   long long total = 0, nctr = 0;
   uint32_t stage_bytes = 0;
+  int max_bn = 32;
   for (int i = 0; i < n; ++i) {
     const TcPlan* p = static_cast<const TcPlan*>(plans[i]);
     if (!p) { delete c; return set_error("gemm_chain_create: plan %d is NULL", i); }
@@ -395,6 +327,7 @@ extern "C" int dlrm_b200_gemm_chain_create(void* const* plans, const int* dep, c
     }
     const uint32_t sb = (uint32_t)((Q.a.x3 ? 2 : 1) * (TC_BM * TC_BK * 2 + Q.bn * TC_BK * 2));
     stage_bytes = sb > stage_bytes ? sb : stage_bytes;
+    max_bn = Q.bn > max_bn ? Q.bn : max_bn;
   }
   // groups (see ChGroup): maximal runs of single-split problems with equal m tiles, m-tile major
   {
@@ -422,15 +355,19 @@ extern "C" int dlrm_b200_gemm_chain_create(void* const* plans, const int* dep, c
   P.n = n;
   P.total = (int)total;
   P.stage_bytes = stage_bytes;
+  P.max_bn = max_bn;
   int budget_kb = get_tunable(TUNE_GEMM_SMEM_KB);
   if (budget_kb <= 0 || budget_kb > 200) budget_kb = 200;
-  int stages = (int)(((size_t)budget_kb * 1024) / stage_bytes);
+  size_t ring_bytes = (size_t)budget_kb * 1024;
+  if (ring_bytes > TC_MAX_SMEM - tc_extra_smem(max_bn, CH_HEAD)) ring_bytes = TC_MAX_SMEM - tc_extra_smem(max_bn, CH_HEAD);
+  int stages = (int)(ring_bytes / stage_bytes);
   if (stages > 8) stages = 8;
   if (stages < 2) stages = 2;
   P.stages = stages;
   P.ctr = counters;
   P.n_ctr = (int)(2 + nctr);
-  c->smem = (size_t)stages * stage_bytes + 512 + CH_EPI_WARPS * TC_EPI_WARP_BYTES + 1024;   // ring | barriers, task ring | staging
+  c->smem = (size_t)stages * stage_bytes + tc_extra_smem(max_bn, CH_HEAD);   // ring | barriers, task ring | accumulator | staging
+  if (c->smem > (size_t)TC_MAX_SMEM) { delete c; return set_error("gemm_chain_create: %zu bytes of shared memory", c->smem); }
   int dev = 0, sms = 0;
   DLRM_CUDA(cudaGetDevice(&dev));
   DLRM_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -463,7 +400,7 @@ extern "C" int dlrm_b200_gemm_chain_run(void* chain, void* stream) {
   Chain* c = static_cast<Chain*>(chain);
   static bool configured = false;
   if (!configured) {
-    DLRM_CUDA(cudaFuncSetAttribute(gemm_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    DLRM_CUDA(cudaFuncSetAttribute(gemm_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_MAX_SMEM));
     configured = true;
   }
   (void)launch_chain(gemm_chain_kernel, dim3(c->grid), dim3(CH_THREADS), c->smem, static_cast<cudaStream_t>(stream), c->P);

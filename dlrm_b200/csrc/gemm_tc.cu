@@ -1,6 +1,6 @@
-// tcgen05 / TMEM / TMA GEMM for the MLP layers (forward, dgrad, wgrad) on sm_100a.
+// wgmma / TMA GEMM for the MLP layers (forward, dgrad, wgrad) on sm_90a.
 //
-//   D[M,N] = sum_k A(m,k) * B(n,k)        bf16 operands, fp32 accumulation in tensor memory.
+//   D[M,N] = sum_k A(m,k) * B(n,k)        bf16 operands, fp32 accumulation in registers.
 //
 // Precision modes
 //   BF16   : one MMA per k-step (operands rounded to bf16).
@@ -11,16 +11,16 @@
 //            measured in tests/test_gpu_gemm_tc.py).  4 operand tiles per stage instead of 2.
 //
 // Structure (one 128 x BN output tile per CTA, optional split-K over gridDim.z):
-//   warp 0     : TMA producer  -- cp.async.bulk.tensor.2d into a 128B-swizzled smem ring, mbarrier
-//                complete_tx signalling.
-//   warp 1     : allocates TMEM, one elected lane issues tcgen05.mma (cta_group::1, kind::f16,
-//                UMMA 128 x BN x 16), tcgen05.commit releases smem stages / publishes the accumulator.
-//   warps 2..5 : epilogue -- tcgen05.ld (32x32b.x32) of their TMEM lane quadrant, fused
-//                activation / activation-gradient mask, then fp32 and/or (hi,lo) bf16 stores in
-//                normal and transposed layout (the operand layouts of the next GEMMs).
+//   warp 0      : TMA producer -- cp.async.bulk.tensor.2d into a 128B-swizzled smem ring, mbarrier
+//                 complete_tx signalling.
+//   warps 4..11 : two consumer warpgroups; warpgroup w issues wgmma.mma_async m64nBNk16 for rows
+//                 [64 w, 64 w + 64) of the tile and releases each ring stage once its wgmmas retire.
+//                 Then the accumulators go through shared memory to the epilogue on the same 8 warps:
+//                 fused bias / activation / activation-gradient mask, fp32 and/or (hi,lo) bf16 stores
+//                 in normal and transposed layout (the operand layouts of the next GEMMs).
 // Operands may be K-major ([rows, K] with K contiguous) or MN-major ([K, rows] with rows
-// contiguous, e.g. dY^T read straight from dY): the UMMA descriptors and instruction descriptor
-// carry the majorness, so no transposed copy is needed for MN-major inputs.
+// contiguous, e.g. dY^T read straight from dY): the smem descriptors and the wgmma transpose
+// immediates carry the majorness, so no transposed copy is needed for MN-major inputs.
 #include <string.h>
 
 #include "gemm_tc_common.cuh"
@@ -91,7 +91,7 @@ template <int BN>
 static int launch_tc(const TcPlan& p, cudaStream_t st) {
   static bool configured = false;
   if (!configured) {
-    DLRM_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    DLRM_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_MAX_SMEM));
     configured = true;
   }
   (void)launch_chain(gemm_tc_kernel<BN>, p.grid, dim3(TC_THREADS), p.smem, st, p.tmAh, p.tmAl, p.tmBh, p.tmBl, p.args, p.stages);
@@ -135,13 +135,16 @@ extern "C" int dlrm_b200_gemm_tc_plan_create(const dlrm_gemm_tc_desc_t* d, void*
     if (d->N <= 32) bn = 32; else if (d->N <= 64 && bn > 64) bn = 64;
   }
   if (a.b_mn && bn < 64) bn = 64;  // MN-major boxes are 64 wide
-  // operand-ring budget: 200 KB = deepest pipeline, one CTA per SM; ~100 KB lets two CTAs (of this or of
-  // a concurrent GEMM on another stream) share an SM, which hides the latency of these small problems
+  // operand-ring budget (default 200 KB, the deepest ring).  The accumulator is staged in the ring once the last
+  // wgmma has retired, so only the barriers and the epilogue's per-warp staging sit beside it.  A smaller budget
+  // no longer lets two CTAs share an SM: 384 threads at ~160 registers take more than half the register file.
   int budget_kb = get_tunable(TUNE_GEMM_SMEM_KB);
   if (budget_kb <= 0 || budget_kb > 200) budget_kb = 200;
   if (budget_kb < 48) budget_kb = 48;
+  const size_t ring_cap = TC_MAX_SMEM - (256 + TC_EPI_BYTES + 1024);
+  const size_t ring_budget = (size_t)budget_kb * 1024 < ring_cap ? (size_t)budget_kb * 1024 : ring_cap;
   if (!(d->tile_n == 128) && bn == 128 &&
-      (size_t)budget_kb * 1024 < 2 * (size_t)(a.x3 ? 2 : 1) * (TC_BM * TC_BK * 2 + 128 * TC_BK * 2))
+      ring_budget < 2 * (size_t)(a.x3 ? 2 : 1) * (TC_BM * TC_BK * 2 + 128 * TC_BK * 2))
     bn = 64;                       // two stages of a 128-wide tile would not fit the budget
   p->bn = bn;
   a.num_kb = (int)((d->K + TC_BK - 1) / TC_BK);
@@ -154,12 +157,14 @@ extern "C" int dlrm_b200_gemm_tc_plan_create(const dlrm_gemm_tc_desc_t* d, void*
     delete p; return set_error("gemm_tc: split-K only supports fp32 slab outputs");
   }
   const size_t stage_bytes = (size_t)(a.x3 ? 2 : 1) * (TC_BM * TC_BK * 2 + bn * TC_BK * 2);
-  int stages = (int)(((size_t)budget_kb * 1024) / stage_bytes);
+  int stages = (int)(ring_budget / stage_bytes);
   if (stages > 8) stages = 8;
   if (stages < 2) stages = 2;
   if (stages > a.kb_per_split) stages = a.kb_per_split < 2 ? 2 : a.kb_per_split;
   p->stages = stages;
-  p->smem = stages * stage_bytes + 256 + TC_EPI_BYTES + 1024;   // ring | barriers (<= 256 B) | epilogue staging
+  // ring (also holds the staged accumulator) | barriers (<= 256 B) | per-warp staging | alignment
+  p->smem = tc_ring_bytes(stages * stage_bytes, bn) + 256 + TC_EPI_BYTES + 1024;
+  if (p->smem > (size_t)TC_MAX_SMEM) { delete p; return set_error("gemm_tc: %zu bytes of shared memory", p->smem); }
   p->grid = dim3((unsigned)((d->N + bn - 1) / bn), (unsigned)mt, (unsigned)splits);
   int rc = 0;
   // operand maps.  K-major: tensor [rows, K]; MN-major: tensor [K, rows].

@@ -1,4 +1,4 @@
-// Body of the tcgen05 GEMM CTA (see gemm_tc.cu for the design).  Textually included by the kernels
+// Body of the wgmma GEMM CTA (see gemm_tc.cu for the design).  Textually included by the kernels
 // that share it; the including kernel provides, as macros or locals:
 //   TCB_BX / TCB_BY / TCB_BZ        tile coordinates (n tile, m tile, k split)
 //   TCB_MAP_AH / _AL / _BH / _BL    const CUtensorMap* of the four operand maps (kernel-parameter space)
@@ -7,12 +7,14 @@
 //   BN      template int            tile width
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  constexpr uint32_t A_BYTES = TC_BM * TC_BK * 2;  // 16 KB
+  constexpr uint32_t A_BYTES = TC_A_BYTES;
   constexpr uint32_t B_BYTES = BN * TC_BK * 2;
   const uint32_t stage_bytes = (g.x3 ? 2u : 1u) * (A_BYTES + B_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)stages * stage_bytes);
-  // bars[0..stages) full, [stages..2*stages) empty, [2*stages] accumulator ready
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * stages + 1);
+  const size_t ring_bytes = tc_ring_bytes((size_t)stages * stage_bytes, BN);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ring_bytes);
+  // bars[0..stages) full, [stages..2*stages) empty
+  float* acc = reinterpret_cast<float*>(smem);   // the ring, once every TMA load has landed and every wgmma retired
+  uint8_t* epi = smem + ring_bytes + 256;
 
   pdl_launch_dependents();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -25,23 +27,12 @@
   if (threadIdx.x == 0) {
     for (int s = 0; s < stages; ++s) {
       mbar_init(bar_base + 8 * s, 1);
-      mbar_init(bar_base + 8 * (stages + s), 1);
+      mbar_init(bar_base + 8 * (stages + s), TC_EPI_WARPS);   // one arrive per consumer warp
     }
-    mbar_init(bar_base + 8 * (2 * stages), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    // allocate BN fp32 accumulator columns (power of two >= 32)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"((uint32_t)(BN < 32 ? 32 : BN))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();   // barriers and TMEM are set up; global memory is first touched below
+  pdl_wait();   // barriers are set up; global memory is first touched below
 
   if (warp == 0) {
     // ------------------------------------------------------------------ TMA producer
@@ -78,63 +69,18 @@
         if (++stage == stages) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    // instruction descriptor: D=f32 (1<<4), A=B=bf16 (1<<7, 1<<10), majorness bits 15/16,
-    // N>>3 at [17,23), M>>4 at [24,29)
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)g.a_mn << 15) |
-                           ((uint32_t)g.b_mn << 16) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
+  } else if (warp >= TC_CONSUMER_WARP0) {
+    // ------------------------------------------------------------------ wgmma consumers + epilogue
+    const int cw = warp - TC_CONSUMER_WARP0;
+    float d[BN / 2];
     int stage = 0;
     uint32_t phase = 0;
-    uint32_t accum = 0;
-    for (int kb = kb0; kb < kb1; ++kb) {
-      mbar_wait(bar_base + 8 * stage, phase);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (lane == 0) {
-        const uint32_t sa_hi = smem_base + stage * stage_bytes;
-        const uint32_t sa_lo = sa_hi + A_BYTES;
-        const uint32_t sb_hi = sa_hi + (g.x3 ? 2u : 1u) * A_BYTES;
-        const uint32_t sb_lo = sb_hi + B_BYTES;
-#pragma unroll
-        for (int k = 0; k < TC_BK / 16; ++k) {
-          // K-major SW128: rows of 128 B, 8-row groups 1024 B apart (SBO), k-step = +32 B.
-          // MN-major SW128: [64 k rows][64 mn] boxes: k-groups 1024 B apart (SBO), 64-wide mn blocks
-          //                 8192 B apart (LBO), k-step (16 rows) = +2048 B.
-          const uint32_t a_off = g.a_mn ? k * 2048u : k * 32u;
-          const uint32_t b_off = g.b_mn ? k * 2048u : k * 32u;
-          const uint32_t a_lbo = g.a_mn ? 8192u : 16u, b_lbo = g.b_mn ? 8192u : 16u;
-          const uint64_t ah = make_smem_desc(sa_hi + a_off, a_lbo, 1024);
-          const uint64_t bh = make_smem_desc(sb_hi + b_off, b_lbo, 1024);
-          if (g.x3) {
-            const uint64_t al = make_smem_desc(sa_lo + a_off, a_lbo, 1024);
-            const uint64_t bl = make_smem_desc(sb_lo + b_off, b_lbo, 1024);
-            umma_bf16(tmem_base, al, bh, idesc, accum);
-            umma_bf16(tmem_base, ah, bl, idesc, 1u);
-            umma_bf16(tmem_base, ah, bh, idesc, 1u);
-          } else {
-            umma_bf16(tmem_base, ah, bh, idesc, accum);
-          }
-          accum = 1u;
-        }
-        umma_commit(bar_base + 8 * (stages + stage));              // smem stage free when MMAs retire
-        if (kb == kb1 - 1) umma_commit(bar_base + 8 * (2 * stages));  // accumulator complete
-      }
-      __syncwarp();
-      if (++stage == stages) { stage = 0; phase ^= 1; }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue (warps 2..)
-    const int quad = warp & 3;  // TMEM lane quadrant this warp may access
-    mbar_wait(bar_base + 8 * (2 * stages), 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    uint8_t* stage_warp = smem + (size_t)stages * stage_bytes + 256 + (size_t)(warp - 2) * TC_EPI_WARP_BYTES;
-    tc_epilogue_tile(g, BN, m0, n0, TCB_BZ, tmem_base, quad, lane, stage_warp, (warp - 2) >> 2, TC_EPI_WARPS / 4);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  }
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"((uint32_t)(BN < 32 ? 32 : BN))
-                 : "memory");
+    tc_mainloop<BN>(d, g, smem_base, stage_bytes, stages, bar_base, bar_base + 8 * stages, kb0, kb1, stage, phase,
+                    cw >> 2, lane);
+    // both warpgroups' wgmmas have retired (every operand the producer loaded was waited for): the ring is free
+    asm volatile("bar.sync 2, %0;" ::"n"(32 * TC_EPI_WARPS) : "memory");
+    tc_stage_acc<BN>(d, acc, cw, lane);
+    asm volatile("bar.sync 1, %0;" ::"n"(32 * TC_EPI_WARPS) : "memory");
+    tc_epilogue_tile(g, BN, m0, n0, TCB_BZ, acc, cw & 3, lane, epi + (size_t)cw * TC_EPI_WARP_BYTES, cw >> 2,
+                     TC_EPI_WARPS / 4);
   }

@@ -1,6 +1,7 @@
-// Shared pieces of the tcgen05 GEMM kernels (gemm_tc.cu: one tile per CTA; gemm_chain.cu: persistent
-// tile-dataflow kernel): tile constants, the problem description, PTX wrappers (mbarrier, TMA, tcgen05),
-// the UMMA shared-memory descriptor and the plan object the C ABI hands out.
+// Shared pieces of the wgmma GEMM kernels (gemm_tc.cu: one tile per CTA; gemm_chain.cu: persistent
+// tile-dataflow kernel): tile constants, the problem description, PTX wrappers (mbarrier, TMA, wgmma),
+// the wgmma shared-memory descriptor, the consumer main loop, the epilogue and the plan object the C ABI
+// hands out.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -11,6 +12,7 @@ namespace dlrm {
 
 constexpr int TC_BM = 128;
 constexpr int TC_BK = 64;  // 64 bf16 = 128 bytes = one swizzle row
+constexpr int TC_MAX_SMEM = 227 * 1024;   // dynamic shared memory one sm_90 block may opt in to
 
 struct TcArgs {
   long long M, N, K;
@@ -75,39 +77,50 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "l"(map), "r"(bar), "r"(x), "r"(y)
       : "memory");
 }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 
-// UMMA shared-memory descriptor (cute::UMMA::SmemDescriptor): start>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version=1 [46,48), layout SWIZZLE_128B=2 [61,64).
+// wgmma.mma_async m64nNk16, bf16 x bf16 -> f32 accumulated in registers (scale-d = 1: the caller zeroes d).
+// TA / TB: operand A / B is MN-major (transposed) in shared memory.  Fragment of thread t of the warpgroup:
+// d[4j + 2h + c] = D[16 (t / 32) + (t % 32) / 4 + 8h][8j + 2 (t % 4) + c].
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[16], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(1), "n"(TA), "n"(TB));
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(1), "n"(TA), "n"(TB));
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(1), "n"(TA), "n"(TB));
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// wgmma shared-memory descriptor (sm_90): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), base offset 0
+// (every tile is 1024-byte aligned), layout SWIZZLE_128B=1 [62,64).
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((addr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
 
@@ -118,28 +131,118 @@ __device__ __forceinline__ float apply_act_tc(float v, int act) {
 }
 
 
+// ------------------------------------------------------------------------------------------ CTA layout
+// Warpgroup 0: warp 0 lane 0 is the TMA producer (warps 1-3 only exist so that the consumers are whole,
+// aligned warpgroups).  Warpgroups 1 and 2 are the consumers: consumer warpgroup w issues the wgmmas of
+// accumulator rows [64 w, 64 w + 64) of the 128 x BN tile, then all 8 consumer warps run the epilogue.
+constexpr int TC_EPI_WARPS = 8;
+constexpr int TC_THREADS = 128 + 32 * TC_EPI_WARPS;
+constexpr int TC_CONSUMER_WARP0 = 4;
+constexpr uint32_t TC_A_BYTES = TC_BM * TC_BK * 2;   // 16 KB; rows 64..127 start at +8 KB in both majornesses
+
+// Consumer main loop over k blocks [kb0, kb1) of one tile.  Every stage of the ring holds A_hi [A_lo] B_hi
+// [B_lo] (x3 adds the lo tiles), each 1024-byte aligned in the 128-byte swizzle TMA writes.  A stage is
+// released (one arrive per consumer warp) once the wgmmas that read it have retired; the wgmmas of the next
+// k block are already issued by then.  `stage` / `phase` carry the ring position across calls.
+//   K-major SW128 : rows of 128 B, 8-row groups 1024 B apart (SBO); a 16-wide k step = +32 B.
+//   MN-major SW128: [64 k rows][64 mn] boxes; 8-row k groups 1024 B apart (SBO), 64-wide mn blocks 8192 B
+//                   apart (LBO); a 16-deep k step = +2048 B.
+template <int BN, int TA, int TB>
+__device__ __forceinline__ void tc_mainloop_t(float (&d)[BN / 2], bool x3, uint32_t ring, uint32_t stage_bytes,
+                                              int stages, uint32_t bar_full, uint32_t bar_empty, int kb0, int kb1,
+                                              int& stage, uint32_t& phase, int wg, int lane) {
+  constexpr uint32_t B_BYTES = BN * TC_BK * 2;
+  constexpr uint32_t a_lbo = TA ? 8192u : 16u, b_lbo = TB ? 8192u : 16u;
+  int prev = -1;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(bar_full + 8 * stage, phase);
+    __syncwarp();
+    const uint32_t sa_hi = ring + stage * stage_bytes + (uint32_t)wg * (TC_A_BYTES / 2);
+    const uint32_t sa_lo = sa_hi + TC_A_BYTES;
+    const uint32_t sb_hi = ring + stage * stage_bytes + (x3 ? 2u : 1u) * TC_A_BYTES;
+    const uint32_t sb_lo = sb_hi + B_BYTES;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < TC_BK / 16; ++k) {
+      const uint32_t a_off = TA ? k * 2048u : k * 32u;
+      const uint32_t b_off = TB ? k * 2048u : k * 32u;
+      const uint64_t ah = make_smem_desc(sa_hi + a_off, a_lbo, 1024);
+      const uint64_t bh = make_smem_desc(sb_hi + b_off, b_lbo, 1024);
+      if (x3) {
+        wgmma_bf16<TA, TB>(d, make_smem_desc(sa_lo + a_off, a_lbo, 1024), bh);
+        wgmma_bf16<TA, TB>(d, ah, make_smem_desc(sb_lo + b_off, b_lbo, 1024));
+      }
+      wgmma_bf16<TA, TB>(d, ah, bh);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();                              // the previous k block's wgmmas have retired
+    if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
+    prev = stage;
+    if (++stage == stages) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
+}
+
+template <int BN>
+__device__ __forceinline__ void tc_mainloop(float (&d)[BN / 2], const TcArgs& g, uint32_t ring,
+                                            uint32_t stage_bytes, int stages, uint32_t bar_full, uint32_t bar_empty,
+                                            int kb0, int kb1, int& stage, uint32_t& phase, int wg, int lane) {
+#pragma unroll
+  for (int j = 0; j < BN / 2; ++j) d[j] = 0.f;
+  const bool x3 = g.x3 != 0;
+  if (!g.a_mn && !g.b_mn)
+    tc_mainloop_t<BN, 0, 0>(d, x3, ring, stage_bytes, stages, bar_full, bar_empty, kb0, kb1, stage, phase, wg, lane);
+  else if (!g.a_mn)
+    tc_mainloop_t<BN, 0, 1>(d, x3, ring, stage_bytes, stages, bar_full, bar_empty, kb0, kb1, stage, phase, wg, lane);
+  else if (!g.b_mn)
+    tc_mainloop_t<BN, 1, 0>(d, x3, ring, stage_bytes, stages, bar_full, bar_empty, kb0, kb1, stage, phase, wg, lane);
+  else
+    tc_mainloop_t<BN, 1, 1>(d, x3, ring, stage_bytes, stages, bar_full, bar_empty, kb0, kb1, stage, phase, wg, lane);
+}
+
 // ------------------------------------------------------------------------------------------ epilogue
-// One accumulator tile (128 rows x bn columns in tensor memory) -> global memory, shared by the per-layer
-// kernel (gemm_tc.cu) and the persistent chain kernel (gemm_chain.cu).
+// The accumulator tile is staged in shared memory as fp32 [128][BN + 4] (the 4-float pad makes the epilogue's
+// row-per-lane 16-byte reads conflict-free), then every consumer warp reads ONE ROW per lane, 32 consecutive
+// columns at a time.
+__host__ __device__ constexpr int tc_acc_ld(int bn) { return bn + 4; }
+__host__ __device__ constexpr int tc_acc_bytes(int bn) { return TC_BM * tc_acc_ld(bn) * 4; }
+
+// consumer warp cw (0..7) stores its wgmma fragment: rows 16 cw + lane / 4 (+ 8), columns 8 j + 2 (lane % 4)
+template <int BN>
+__device__ __forceinline__ void tc_stage_acc(const float (&d)[BN / 2], float* acc, int cw, int lane) {
+  float* r0 = acc + (size_t)(16 * cw + (lane >> 2)) * tc_acc_ld(BN) + 2 * (lane & 3);
+  float* r1 = r0 + 8 * tc_acc_ld(BN);
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    *reinterpret_cast<float2*>(r0 + 8 * j) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(r1 + 8 * j) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
+}
+
+// Staged tile (128 rows x bn columns) -> global memory, shared by the per-layer kernel (gemm_tc.cu) and the
+// persistent chain kernel (gemm_chain.cu).
 //
-// tcgen05.ld hands every thread ONE ROW (32 consecutive columns per load).  Storing from that layout makes
-// each warp-wide 16-byte store hit 32 different rows (32 half-written sectors per instruction); measured with
-// the chain kernel's per-task timeline (tools/chain_timeline.py, profiles/r2_chain_timeline_before.txt) that
-// cost 10-19 us per 128 x 128 tile -- more than the tile's MMAs.  Here every 32 x 32 chunk is transposed
-// through a per-warp shared-memory tile (padded rows: conflict-free 16-byte accesses) so that a warp store
-// covers whole row segments: 8 rows x 64 B for the bf16 (hi, lo) operands, 4 rows x 128 B for fp32; the
-// activation-gradient mask is read the same way.  Chunks that are ragged (N tail, the diverted bias-gradient
-// column) or whose rows are not 16-byte aligned use element-wise but still row-contiguous accesses.
+// Storing straight from the row-per-lane layout would make each warp-wide 16-byte store hit 32 different rows
+// (32 half-written sectors per instruction).  Instead every 32 x 32 chunk is transposed through a per-warp
+// shared-memory tile (padded rows: conflict-free 16-byte accesses) so that a warp store covers whole row
+// segments: 8 rows x 64 B for the bf16 (hi, lo) operands, 4 rows x 128 B for fp32; the activation-gradient
+// mask is read the same way.  Chunks that are ragged (N tail, the diverted bias-gradient column) or whose rows
+// are not 16-byte aligned use element-wise but still row-contiguous accesses.
 constexpr int TC_EPI_ROW_F32 = 20;                 // floats per staged fp32 half-row (16 + 4 pad)
 constexpr int TC_EPI_ROW_BF16 = 40;                // bf16 per staged bf16 row (32 + 8 pad)
 constexpr int TC_EPI_WARP_BYTES = 32 * TC_EPI_ROW_BF16 * 2;  // 2560 B per epilogue warp (fp32: two 16-column passes)
-// Epilogue warps per CTA: two per TMEM lane quadrant (warps w and w + 4 may both read quadrant w % 4) split the
-// 32-column chunks of a tile.  The epilogue is a long dependent instruction stream per warp (tcgen05.ld -> convert
-// -> shared-memory transpose -> store) with ONE warp per scheduler, i.e. issue-latency bound: a second warp per
-// scheduler halves it (chain timeline: 4-10 us -> 3-6 us per tile).
-constexpr int TC_EPI_WARPS = 8;
-constexpr int TC_THREADS = 64 + 32 * TC_EPI_WARPS;       // warp 0: TMA, warp 1: MMA, then the epilogue warps
 constexpr int TC_EPI_BYTES = TC_EPI_WARPS * TC_EPI_WARP_BYTES;
+// persistent chain kernel: dynamic shared memory besides the operand ring (its producer streams the next task's
+// operands while the epilogue runs, so the accumulator needs a region of its own):
+// barriers + task ring | accumulator | per-warp staging | align
+__host__ __device__ constexpr size_t tc_extra_smem(int bn, int head) {
+  return (size_t)head + tc_acc_bytes(bn) + TC_EPI_BYTES + 1024;
+}
+// per-layer kernel: the accumulator is staged in the operand ring, idle once the last wgmma has retired
+__host__ __device__ constexpr size_t tc_ring_bytes(size_t ring, int bn) {
+  return ring > (size_t)tc_acc_bytes(bn) ? ring : (size_t)tc_acc_bytes(bn);
+}
 
 // 32 x 32 bf16 chunk, one row per thread in `mine` -> global rows [mrow0, mrow0 + 32) x columns [nb, nb + 32)
 __device__ __forceinline__ void tc_epi_store_bf16(const __nv_bfloat16 (&mine)[32], __nv_bfloat16* dst, long long ld,
@@ -166,13 +269,13 @@ __device__ __forceinline__ void tc_epi_store_bf16(const __nv_bfloat16 (&mine)[32
   __syncwarp();
 }
 
-// c0 / cstep: this warp handles the 32-column chunks c0, c0 + cstep, ... (two warps per TMEM lane quadrant split
-// the chunks of a tile between them in the chain kernel; the per-layer kernel passes 0, 1).
-__device__ __forceinline__ void tc_epilogue_tile(const TcArgs& g, int bn, int m0, int n0, int bz, uint32_t tmem_acc,
-                                                 int quad, int lane, uint8_t* stage_warp, int c0 = 0, int cstep = 1) {
+// This warp handles rows [32 quad, 32 quad + 32) of the tile and its 32-column chunks c0, c0 + cstep, ... (two
+// warps per 32-row block split the chunks of a tile between them).
+__device__ __forceinline__ void tc_epilogue_tile(const TcArgs& g, int bn, int m0, int n0, int bz, const float* acc,
+                                                 int quad, int lane, uint8_t* stage_warp, int c0, int cstep) {
   // Every field is copied into a register ONCE: `g` lives in kernel-parameter space (indexed at run time in the
-  // chain kernel) and the tcgen05 / mbarrier asm statements clobber memory, so reading g.act or g.bias inside the
-  // element loops costs a constant-bank load + a branch PER ELEMENT (measured: 3-7 us per 32 x 32 chunk).
+  // chain kernel) and the mbarrier asm statements clobber memory, so reading g.act or g.bias inside the
+  // element loops costs a constant-bank load + a branch PER ELEMENT.
   const long long M = g.M, N = g.N;
   const int act = g.act, mask_act = g.mask_act;
   const __nv_bfloat16* const mask_hi = g.mask_hi;
@@ -204,7 +307,13 @@ __device__ __forceinline__ void tc_epilogue_tile(const TcArgs& g, int bn, int m0
     const long long nb = (long long)n0 + c * 32;
     if (nb >= N) break;
     uint32_t r[32];
-    tmem_ld32(tmem_acc + ((uint32_t)(quad * 32) << 16) + (uint32_t)(c * 32), r);
+    const float4* arow = reinterpret_cast<const float4*>(acc + (size_t)(quad * 32 + lane) * tc_acc_ld(bn) + c * 32);
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const float4 t = arow[q];
+      r[4 * q] = __float_as_uint(t.x); r[4 * q + 1] = __float_as_uint(t.y);
+      r[4 * q + 2] = __float_as_uint(t.z); r[4 * q + 3] = __float_as_uint(t.w);
+    }
     float v[32];
     const bool full = nb + 32 <= N;
 #pragma unroll

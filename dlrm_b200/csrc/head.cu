@@ -174,7 +174,7 @@ extern "C" int dlrm_b200_head_fused(const float* h, int64_t ldh, const float* w,
   a.partial = scratch ? reinterpret_cast<float*>(static_cast<char*>(scratch) + 16) : nullptr;
   a.B = batch; a.K = (int)K; a.act_last = act_last; a.act_prev = act_prev; a.loss_kind = loss_kind;
   a.thr = loss_threshold;
-  // 16 samples per CTA: 128 CTAs at batch 2048 (one wave of the 148 SMs) instead of 64
+  // 16 samples per CTA: 128 CTAs at batch 2048 (about one wave of the 132 SMs) instead of 64
   const int rows = get_tunable(TUNE_HEAD_ROWS) == 32 ? 32 : 16;
   const long long nb = (batch + rows - 1) / rows;
   if (rows == 32) (void)launch_chain(head_kernel<32>, dim3((unsigned)nb), dim3(256), 0, static_cast<cudaStream_t>(stream), a);

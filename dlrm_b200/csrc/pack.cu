@@ -1,4 +1,4 @@
-// Operand preparation for the tcgen05 GEMMs.
+// Operand preparation for the wgmma GEMMs.
 //   split_bf16       : fp32 [M,N] -> (hi, lo) bf16 pairs, hi = bf16(x), lo = bf16(x - hi)
 //   dense_update_pack: dense branch of optimizer.step() (torch.optim.SGD / optim/rwsadagrad.py:145-148)
 //                      fused with the split-K slab reduction of the weight gradients and with the

@@ -1,4 +1,4 @@
-"""`DLRM_Net` -- the reference's module surface (dlrm_s_pytorch.py:207-730) over the B200 engine.
+"""`DLRM_Net` -- the reference's module surface (dlrm_s_pytorch.py:207-730) over the H100 engine.
 
 Call-compatible with the reference for the hot path (SURVEY.md §8 b1):
   * constructor keyword signature of `dlrm_s_pytorch.py:296-317` (no-arg construction allowed);

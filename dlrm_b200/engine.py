@@ -1,4 +1,4 @@
-"""Device-side engine of the DLRM hot path on one B200.
+"""Device-side engine of the DLRM hot path on one H100.
 
 Owns the HBM layout (one table arena, one dense-parameter arena, activation/gradient buffers
 written in place by the producing kernels) and sequences the C-ABI kernels of
@@ -74,7 +74,7 @@ class Engine:
                  max_batch: int = 2048, gemm: str = "simt", n_features: Optional[int] = None,
                  interleave_momentum: Optional[bool] = None, shards=None, split_slots=None, small_rows_max: int = 256):
         if not torch.cuda.is_available():
-            raise RuntimeError("dlrm_b200.Engine needs a CUDA device (B200, sm_100a); there is no CPU path")
+            raise RuntimeError("dlrm_b200.Engine needs a CUDA device (H100, sm_90a); there is no CPU path")
         self.device = torch.device(device)
         self.lib = _lib.lib()
         sm, major, minor = _lib.device_info(self.device.index or 0)
@@ -119,7 +119,7 @@ class Engine:
         self.gemm = GEMM_SIMT_FP32          # back end of the fp32-pointer entry points
         self.tc = gemm != "simt"
         self.tc_x3 = 1 if gemm == "tc" else 0
-        self.tc_B = -1                       # batch size the tcgen05 plans were built for
+        self.tc_B = -1                       # batch size the wgmma plans were built for
         self._pack_dirty = True
         if self.ln_bot[-1] != self.D:
             raise ValueError("bottom MLP output %d != sparse feature size %d" % (self.ln_bot[-1], self.D))
@@ -137,10 +137,9 @@ class Engine:
         self.total_rows = int(self.row_base[-1])
         # Row layout.  interleave (default when D % 4 == 0): [D weights | Adagrad accumulator | list head (int32) |
         # 2 pad], row stride D + 4 floats -- the two per-row words of the backward live in the row's own DRAM page.
-        # Measured (profiles/README.md, r2_12): the update kernel is bound by the RATE of random DRAM accesses
-        # (~10 G/s: a 4-byte head[] read costs what a 512-byte row costs); dropping the weight-row traffic
-        # entirely only saved 26 %, the separate head / accumulator arrays are the rest.  The gather pays a few
-        # points of bandwidth for rows that are no longer 512-byte aligned (528-byte stride).
+        # The update kernel is bound by the RATE of random DRAM accesses, not by bytes: a 4-byte head[] read costs
+        # about what a 512-byte row costs, so separate head / accumulator arrays would add two random accesses per
+        # row.  The gather pays a little bandwidth for rows that are no longer 512-byte aligned (528-byte stride).
         # interleave=False: dense [rows, D] tables + separate accumulator / head arrays (round 1's layout).
         if interleave_momentum is None:
             interleave_momentum = (self.D % 4 == 0) and os.environ.get("DLRM_ROW_META", "1") != "0"
@@ -201,13 +200,12 @@ class Engine:
         self.multi_stream = True
         # DLRM_CHAIN=1: every MLP chain (forward layers; dgrad chain + weight gradients) as ONE persistent
         # tile-dataflow launch (csrc/gemm_chain.cu) instead of one launch per layer.  Bit-identical results
-        # (tests/test_gpu_chain.py); measured SLOWER inside the step at batch 2048 (profiles/README.md: a CTA
-        # that claimed a task whose producer tiles are not done blocks instead of taking ready work, and the
-        # persistent grid shares the SMs badly with the gather / update kernels of the embedding stream), so
-        # per-layer launches (+ programmatic dependent launch) stay the default.
+        # (tests/test_gpu_chain.py).  Opt-in: a CTA that claimed a task whose producer tiles are not done blocks
+        # instead of taking ready work, and the persistent grid shares the SMs with the gather / update kernels of
+        # the embedding stream, so per-layer launches (+ programmatic dependent launch) stay the default.
         self.use_chain = os.environ.get("DLRM_CHAIN", "0") == "1"
-        self.tc_tile_n = {}          # optional (kind, which, i) -> tile_n override for the tcgen05 plans
-        self.tc_smem_kb = (0, 0)    # (forward, backward) operand-ring budget of the tcgen05 GEMM plans, KB; 0 = 200
+        self.tc_tile_n = {}          # optional (kind, which, i) -> tile_n override for the wgmma plans
+        self.tc_smem_kb = (0, 0)    # (forward, backward) operand-ring budget of the wgmma GEMM plans, KB; 0 = deepest
         self.s_emb = torch.cuda.Stream(device=self.device)
         self.s_wg = torch.cuda.Stream(device=self.device)
         self.s_small = torch.cuda.Stream(device=self.device)
@@ -241,10 +239,9 @@ class Engine:
         self.scratch = torch.zeros(1024, dtype=f32, device=dev)
         self.link = None  # int32 [2 * nnz capacity]
         self.dedup, self._filtered = None, False
-        # Optional duplicate filter for the training gather / update (dlrm_emb_dedup_t).  Measured on B200
-        # (profiles/, r8): it removes the list-head traffic from the update but adds a memset + two small
-        # launches to the gather side and the update time does not move (110 us in-step either way: the
-        # row read-modify-write and the momentum accesses dominate), so it is OFF by default.
+        # Optional duplicate filter for the training gather / update (dlrm_emb_dedup_t).  It removes the list-head
+        # traffic from the update but adds a memset + two small launches to the gather side, while the row
+        # read-modify-write and the accumulator accesses dominate the update; OFF by default.
         self.use_filter = False
 
     def is_small(self, j: int) -> bool:
@@ -607,7 +604,7 @@ class Engine:
         return p
 
     def prepare(self, sp: SparseInput, train: bool = True, batch: Optional[int] = None):
-        """Allocate every lazily-created buffer / tcgen05 plan for this batch shape (no kernels that
+        """Allocate every lazily-created buffer / wgmma plan for this batch shape (no kernels that
         change parameters): required before CUDA-graph capture."""
         B = batch if batch is not None else sp.batch
         if B > self.max_batch:
@@ -918,7 +915,7 @@ class Engine:
                 self.emb_update(sp, optimizer=optimizer, lr=clr, eps=eps)
         self.dense_apply(optimizer, clr, eps)
 
-    # ================================================================== tcgen05 path
+    # ================================================================== wgmma path
     # Layers whose output width is >= 16 run on tensor cores (all bottom layers, the top layers
     # up to the final 256 -> 1 layer, which stays on the fp32 CUDA-core kernels).  Every fp32
     # activation / gradient / weight is kept as a (hi, lo) bf16 pair, activations carry a
@@ -1006,9 +1003,8 @@ class Engine:
                 Ws.append((torch.zeros((N, Kp), dtype=bf, device=dev), torch.zeros((N, Kp), dtype=bf, device=dev), Kp))
             self.tc_in[which], self.tc_gz[which], self.tc_W[which] = ins, gzs, Ws
         FD = self.F * self.D
-        # operand-ring budget per GEMM CTA (KB; 0 = library default 200 = one CTA per SM).  The backward
-        # GEMMs run two at a time (dgrad chain beside the wgrad stream): a ~100 KB ring lets two CTAs share
-        # an SM.  Measured choice, see DESIGN.md section 8.
+        # operand-ring budget per GEMM CTA (KB; 0 = library default 200, the deepest ring).  A smaller ring only
+        # shortens the pipeline: a wgmma CTA (384 threads, ~160 registers) leaves no room for a second one on the SM.
         fwd_kb = int(os.environ.get("DLRM_TC_FWD_SMEM_KB", self.tc_smem_kb[0]))
         bwd_kb = int(os.environ.get("DLRM_TC_BWD_SMEM_KB", self.tc_smem_kb[1]))
 

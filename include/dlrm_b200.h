@@ -1,5 +1,5 @@
 /*
- * dlrm_b200.h -- C ABI of libdlrm_b200.so: the B200 (sm_100a) kernels behind the
+ * dlrm_b200.h -- C ABI of libdlrm_b200.so: the H100 (sm_90a) kernels behind the
  * DLRM_Net forward/backward hot path of facebookresearch/dlrm.
  *
  * The reference has NO native interface for this path: every op below replaces an
@@ -50,7 +50,7 @@ const char* dlrm_b200_last_error(void);
  * index outside its table since the last check.  The only hidden state of the library: 256 bytes of device
  * memory per GPU, allocated on first use. */
 int dlrm_b200_check_device_errors(void* stream);
-/* sm count / compute capability of `device`; error unless cc >= 10.0 */
+/* sm count / compute capability of `device`; error unless cc == 9.0 (the library is built for sm_90a) */
 int dlrm_b200_device_info(int device, int* sm_count, int* cc_major, int* cc_minor);
 /* Experiment knobs of the kernels (ids: csrc/common.cuh `enum Tunable`; dlrm_b200/_lib.py TUNE; env DLRM_TUNE).
  * Process-wide, read at launch time; 0 restores the default of every knob.  Not part of the reference's surface. */
@@ -98,7 +98,8 @@ int dlrm_b200_emb_bag_fwd(const dlrm_emb_fwd_table_t* tables /*[host]*/, int num
  * per-row list: prev = atomicExch(&head[row], pos+1); next[pos] = prev.  `head` is an int32
  * array over all rows of the table, zero on entry and zero again after step 2.
  * Step 2, dlrm_b200_emb_bwd_update: one warp per bag; the list head (= unique owner of a row)
- * sums dY over the row's occurrences in ascending position (== grad.coalesce()), then
+ * sums dY over the row's occurrences: up to 32 in ascending position (== grad.coalesce()), more
+ * with an order-independent fixed-point sum (the same result on every run), then
  *   RWSAdagrad: momentum[row] += mean_d(g^2); W[row] -= lr * g / (sqrt(momentum[row]) + eps)
  *   SGD:        W[row] -= lr * g
  * `lr` is the already-decayed clr of optim/rwsadagrad.py:115.
@@ -117,7 +118,7 @@ typedef struct {
   int64_t mom_stride;   /* elements between consecutive rows' accumulators in `momentum`; 0 = 1.
                          * ld = dim + 4 with momentum = weight + dim and mom_stride = ld keeps the
                          * row-wise Adagrad accumulator in the SAME DRAM burst as its row: the update then
-                         * costs one activation per row instead of two (measured: profiles/). */
+                         * costs one activation per row instead of two. */
   /* Sharded placement.  use_dy_off != 0: the gradient row of (bag b, this table) is at dY(b) + dy_off instead
    * of dY(b) + k*dy_stride_table.  row_n > 0: `weight`/`momentum`/`head` hold rows [row_lo, row_lo + row_n)
    * of the table; occurrences of other rows are another shard's.  head == NULL: this table is not linked and
@@ -245,7 +246,7 @@ int dlrm_b200_linear_wgrad(const float* dY, int64_t lddy, const float* X, int64_
  * ------------------------------------------------------------------------------------------ */
 int dlrm_b200_interact_fwd(const float* T, int64_t ldt, float* R, int64_t ldr, int64_t batch,
                            int num_features, int dim, int itself, void* stream);
-/* _ex variants: additionally emit the (hi, lo) bf16 operand pair consumed by the tcgen05 GEMMs
+/* _ex variants: additionally emit the (hi, lo) bf16 operand pair consumed by the wgmma GEMMs
  * (R for the first top-MLP layer; feature 0 of dT for the bottom MLP's backward).  R may be NULL
  * when only the bf16 pair is wanted. */
 int dlrm_b200_interact_fwd_ex(const float* T, int64_t ldt, float* R, int64_t ldr, void* R_hi, void* R_lo,
@@ -315,8 +316,8 @@ int dlrm_b200_dense_update(float* param, const float* grad, float* state /*NULL 
 
 
 /* ------------------------------------------------------------------------------------------
- * tcgen05 GEMM back end of apply_mlp and its autograd (aten::addmm, dlrm_s_pytorch.py:399-405):
- *   D[M,N] = sum_k A(m,k) * B(n,k),  bf16 operands staged by TMA, fp32 accumulation in TMEM.
+ * wgmma GEMM back end of apply_mlp and its autograd (aten::addmm, dlrm_s_pytorch.py:399-405):
+ *   D[M,N] = sum_k A(m,k) * B(n,k),  bf16 operands staged by TMA, fp32 accumulation in registers.
  * Operands are (hi, lo) bf16 pairs of fp32 values (hi = bf16(x), lo = bf16(x - hi)); mode_x3
  * computes hi*hi + hi*lo + lo*hi (fp32-grade), otherwise hi*hi only.  An operand is K-major
  * ([rows, K], ld = row stride) or MN-major ([K, rows]); ld in elements, multiple of 8.
@@ -352,8 +353,8 @@ int dlrm_b200_gemm_tc_plan_destroy(void* plan);
 /* A whole MLP chain in ONE persistent launch (apply_mlp: `layers(x)`, dlrm_s_pytorch.py:399-405, and its
  * autograd: the dgrad chain with every weight-gradient GEMM beside it, :1613).  The plans' output tiles form
  * one topologically ordered task list (plan order; inside a plan: n tile, m tile, k split); one CTA per SM
- * claims tasks from a device-side queue and runs TMA -> tcgen05.mma -> epilogue with up to 4 accumulators
- * in tensor memory, so the epilogue of a tile overlaps the MMAs of the next.  dep[i] >= 0 names the plan
+ * claims tasks from a device-side queue and runs TMA -> wgmma -> epilogue; the TMA producer already
+ * streams the next tile's operands while the consumers run the epilogue of this one.  dep[i] >= 0 names the plan
  * that produces plan i's A operand inside this launch: a task waits until every 128-row block of that
  * producer covering its A rows (dep_on_k[i] = 0: the task's own m tile; = 1: the task's k range, i.e. a
  * weight-gradient GEMM reducing over the batch) is complete (per-block counters, release/acquire at GPU

@@ -38,6 +38,7 @@ assert os.path.realpath(os.path.dirname(R.__file__)) == os.path.realpath(REF), \
 assert hasattr(R, "DLRM_Net")
 
 from oracle import dlrm_numpy as O  # noqa: E402
+from oracle.golden_format import shrink  # noqa: E402
 
 OUT = os.environ.get("DLRM_GOLDEN_OUT", os.path.join(ROOT, "tests", "golden"))
 
@@ -87,7 +88,7 @@ def stages(ref, X, lS_o, lS_i):
 
 def case(name, m_spa, ln_emb, ln_bot, top_tail, B, lmax, loss, seed, nsteps=2, lr=0.1,
          store_params=True, itself=False, thr=0.0, op="dot", weighted=None, fixed=False,
-         store_tables=None):
+         store_tables=None, shrunk=False):
     ln_emb = list(ln_emb)
     nf = len(ln_emb) + 1
     if op == "dot":
@@ -190,9 +191,10 @@ def case(name, m_spa, ln_emb, ln_bot, top_tail, B, lmax, loss, seed, nsteps=2, l
         with torch.no_grad():
             d[f"{optname}_p_after"] = ref(X, lS_o, lS_i).numpy().copy()
         snapshot(optname, ref, opt, nsteps)
-    path = os.path.join(OUT, name + ".npz")
-    np.savez_compressed(path, **d)
-    _print(f"wrote {path}  ({os.path.getsize(path) / 1e6:.2f} MB)  loss0={d['f_loss']:.6f}")
+    for suffix, arrays in (shrink(d) if shrunk else {"": d}).items():
+        path = os.path.join(OUT, name + suffix + ".npz")
+        np.savez_compressed(path, **arrays)
+        _print(f"wrote {path}  ({os.path.getsize(path) / 1e6:.2f} MB)  loss0={d['f_loss']:.6f}")
 
 
 def embbag_order_check():
@@ -232,7 +234,7 @@ def _main_cases(case):
     case("tiny_default", 2, [4, 3, 2], [4, 3, 2], [4, 2, 1], B=5, lmax=3, loss="mse", seed=11)
     # CFG0 (BASELINE.json configs[0])
     case("cfg0", 16, [1000, 1000, 1000], [13, 512, 256, 64, 16], [512, 256, 1], B=128, lmax=10,
-         loss="bce", seed=22)
+         loss="bce", seed=22, shrunk=True)
     # CFG0 variants: diagonal-inclusive interaction + loss threshold; cat op; weighted pooling
     case("cfg0_itself_thr", 16, [1000, 800, 600], [13, 64, 16], [64, 1], B=64, lmax=10, loss="bce",
          seed=33, itself=True, thr=0.45)
@@ -241,7 +243,7 @@ def _main_cases(case):
          seed=55, weighted="fixed")
     # CFG1/2 shapes (D=128, T=26, same MLPs) with shrunk row counts and batch
     case("mini_cfg1", 128, [2000] * 25 + [40], [13, 512, 256, 128], [1024, 512, 256, 1], B=96,
-         lmax=10, loss="bce", seed=66, store_params=False, store_tables=(0, 13, 25))
+         lmax=10, loss="bce", seed=66, store_params=False, store_tables=(0, 13, 25), shrunk=True)
 
 
 if __name__ == "__main__":

@@ -10,12 +10,12 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (B200); run with -m gpu")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (H100); run with -m gpu")
 
 
 def pytest_collection_modifyitems(config, items):
     """GPU tests are skipped (not failed) when no device is visible, so a bare
-    `pytest tests/` works in the CPU container.  `-m gpu` on a GPU box runs them."""
+    `pytest tests/` works on a machine without a GPU.  `-m gpu` on a GPU box runs them."""
     try:
         import torch
 

@@ -1,4 +1,4 @@
-"""Exhaustive check of the tcgen05 GEMM (dlrm_b200_gemm_tc_*) against float64 references.
+"""Exhaustive check of the wgmma GEMM (dlrm_b200_gemm_tc_*) against float64 references.
 Usable as a CLI (full table, never stops at the first failure -- one GPU call tells everything):
 
     python tests/gemm_tc_check.py [report.txt]

@@ -1,4 +1,5 @@
-"""Loader for tests/golden/*.npz (written by oracle/make_goldens.py from the live reference)."""
+"""Loader for tests/golden/*.npz (written by oracle/make_goldens.py from the live reference; the storage of the
+larger cases is described in oracle/golden_format.py)."""
 import os
 import sys
 
@@ -17,7 +18,11 @@ ALL_CASES = ["tiny_default", "cfg0", "cfg0_itself_thr", "cfg0_cat", "cfg0_weight
 class Golden:
     def __init__(self, name):
         self.name = name
-        z = np.load(os.path.join(GOLDEN_DIR, name + ".npz"))
+        z = dict(np.load(os.path.join(GOLDEN_DIR, name + ".npz")))
+        for part in ("_sgd", "_rwsadagrad"):      # optimizer-step records stored beside the case
+            path = os.path.join(GOLDEN_DIR, name + part + ".npz")
+            if os.path.exists(path):
+                z.update(np.load(path))
         self.z = z
         self.m_spa = int(z["m_spa"])
         self.ln_emb = [int(v) for v in z["ln_emb"]]
@@ -62,7 +67,13 @@ class Golden:
         return dict(op=self.op, itself=self.itself, loss_threshold=self.thr)
 
     def has(self, key):
-        return key in self.z.files
+        return key in self.z
+
+    def dense_grad(self, key, got):
+        """(got, want) for the dense gradient `key`: whole arrays, or both at the stored sample of entries."""
+        if key in self.z:
+            return got, self.z[key]
+        return np.asarray(got).ravel()[self.z[key + "_idx"]], self.z[key + "_val"]
 
     def __getitem__(self, key):
         return self.z[key]

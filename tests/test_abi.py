@@ -32,10 +32,11 @@ def test_abi_version_and_error_text():
     assert b"num_tables" in lib.dlrm_b200_last_error()
 
 
-def test_built_for_sm100a_only():
-    out = os.popen("cuobjdump -lelf %s 2>/dev/null" % _build.LIB).read()
-    assert "sm_100a" in out
-    assert "sm_90" not in out and "sm_80" not in out
+def test_built_for_sm90a_only():
+    cuobjdump = os.path.join(os.path.dirname(_build.nvcc_path()), "cuobjdump")
+    out = os.popen("%s -lelf %s 2>/dev/null" % (cuobjdump, _build.LIB)).read()
+    assert "sm_90a" in out
+    assert "sm_100" not in out and "sm_80" not in out
 
 
 def test_product_does_not_import_oracle():

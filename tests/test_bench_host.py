@@ -1,8 +1,9 @@
-"""bench.py host logic that runs without a GPU: the stage watchdog and the ncu-summary reader."""
+"""bench.py host logic that runs without a GPU: the stage watchdog and the control flow on fakes."""
 import json
 import os
 import subprocess
 import sys
+import types
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -41,17 +42,6 @@ def test_watchdog_without_a_measurement_exits_nonzero_with_an_error_line():
     assert r.returncode == 3
     line = json.loads(r.stdout.strip().splitlines()[-1])
     assert line["value"] is None and "stalled" in line["error"]
-
-
-def test_ncu_summary_reader():
-    sys.path.insert(0, ROOT)
-    import bench
-
-    g = bench.ncu_traffic("emb_fwd_vec_kernel")
-    u = bench.ncu_traffic("emb_update_lean_kernel")
-    assert g is not None and 0.9e9 < g < 1.3e9          # training gather, cfg3: ~1.08 GB of DRAM traffic per launch
-    assert u is not None and 1.5e9 < u < 2.2e9
-    assert bench.ncu_traffic("no_such_kernel") is None
 
 
 def test_bench_flow_on_fakes(monkeypatch, capsys, tmp_path):
@@ -190,7 +180,7 @@ def test_bench_flow_on_fakes(monkeypatch, capsys, tmp_path):
     out = tmp_path / "phases.json"
     args = types.SimpleNamespace(workload="cfg3", gemm="tc", split_forward="partial", ring=2, steps=4, warmup=3,
                                  no_graph=False, no_check=False, no_cpu=False, cpu_budget=1.0, phases=2,
-                                 phases_out=str(out), gpus=1, impl="ours")
+                                 phases_out=str(out), gpus=1, impl="ours", dump_outputs=None)
     bench.ours(args, bench.workload("cfg3", 1))
     cap = capsys.readouterr()
     lines = [ln for ln in cap.out.splitlines() if ln.startswith("{")]
@@ -206,3 +196,39 @@ def test_bench_flow_on_fakes(monkeypatch, capsys, tmp_path):
     assert "parity check" in cap.err and "teardown" in cap.err and "phases {" in cap.err
     ph = json.loads(out.read_text())
     assert [m[0] for m in ph["marks"]] == ["index_exchange", "begin", "emb:update", "step_end"]
+
+
+def test_dump_outputs_writes_the_step_arrays(tmp_path):
+    """bench.dump_outputs on a CPU stand-in of the engine: one float32 / float64 .npy per array, the fixed row
+    sample, and well under the 64 MB cap at the cfg3 model's size."""
+    import numpy as np
+    import torch
+
+    sys.path.insert(0, ROOT)
+    import bench
+
+    D, rows, B = 128, 1000, 8192
+    eng = types.SimpleNamespace(D=D, total_rows=rows, top_act=[torch.rand(B, 1)], dense=torch.rand(2368900),
+                                tables=torch.rand(rows, D + 4))
+    eng.momentum = eng.tables[:, D]
+    bench.dump_outputs(str(tmp_path), eng, torch.tensor([0.5]), B, True)
+    files = sorted(p.name for p in tmp_path.iterdir())
+    assert files == ["dense_params.npy", "emb_accumulator.npy", "emb_row_index.npy", "emb_rows.npy", "loss.npy", "p.npy"]
+    total = 0
+    for f in files:
+        a = np.load(tmp_path / f)
+        assert a.dtype in (np.float32, np.float64), (f, a.dtype)
+        total += a.nbytes
+    assert total < 64 << 20
+    idx = np.load(tmp_path / "emb_row_index.npy").astype(np.int64)
+    assert idx.shape == (bench.DUMP_ROWS,)
+    np.testing.assert_array_equal(np.load(tmp_path / "emb_rows.npy"), eng.tables[torch.from_numpy(idx), :D].numpy())
+    bench.dump_outputs(str(tmp_path / "again"), eng, torch.tensor([0.5]), B, True)
+    np.testing.assert_array_equal(np.load(tmp_path / "again" / "emb_row_index.npy"), idx)   # the same sample every run
+
+
+def test_bench_rejects_zero_steps_and_dumps_without_the_gpu_path():
+    for extra in (["--steps", "0"], ["--impl", "reference", "--dump-outputs", "x"]):
+        r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py")] + extra, capture_output=True, text=True,
+                           timeout=120)
+        assert r.returncode == 2 and "error" in r.stderr, (extra, r.stderr[-500:])

@@ -1,4 +1,4 @@
-"""Persistent tile-dataflow MLP chains (csrc/gemm_chain.cu) == one tcgen05 launch per layer, bit for bit:
+"""Persistent tile-dataflow MLP chains (csrc/gemm_chain.cu) == one wgmma launch per layer, bit for bit:
 same CTA program per tile, so every activation, gradient operand and weight-gradient slab must be identical.
 (Parity of the per-layer path with the reference is tests/test_gpu_engine_tc.py / test_gpu_gemm_tc.py.)"""
 import os
@@ -53,8 +53,7 @@ def _run(use_chain, D, ln_emb, ln_bot, ln_top, B, tile_n=None, steps=2, seed=0):
 CASES = [
     # D, ln_emb, ln_bot, ln_top tail, B
     (128, [1000] * 4, [13, 512, 256, 128], [1024, 512, 256, 1], 2048),
-    (128, [900, 700, 500], [13, 64, 128], [96, 64, 1], 300),      # ragged last m tile, narrow layers (no row
-    # with > 32 occurrences: the update kernel's summation order for longer lists depends on arrival order)
+    (128, [900, 700, 500], [13, 64, 128], [96, 64, 1], 300),      # ragged last m tile, narrow layers
     (16, [1000, 1000, 1000], [13, 512, 256, 64, 16], [512, 256, 1], 128),   # CFG0 shapes
 ]
 

@@ -227,7 +227,8 @@ def test_cli_test_pass_and_checkpoint_follow_the_reference(tmp_path):
 def test_cli_loads_a_reference_checkpoint_for_inference():
     """A checkpoint WRITTEN BY THE REFERENCE (tests/golden/cli_cfg0_C_ref.pt) loads through --load-model
     --inference-only; the test pass gives the accuracy the reference recorded in it."""
-    flags = ["--round-targets=True", "--loss-function=bce"]
+    flags = [f for f in open(os.path.join(ROOT, "tests", "golden", "cli_cfg0_C.flags")).read().split()
+             if not f.startswith("--test-freq")]       # the checkpoint's architecture, no test pass while training
     ck = os.path.join(ROOT, "tests", "golden", "cli_cfg0_C_ref.pt")
     cmd = [sys.executable, os.path.join(ROOT, "dlrm_s_pytorch.py")] + _CLI_BASE + flags + \
         ["--load-model=" + ck, "--inference-only"]

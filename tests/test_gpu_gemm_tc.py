@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (TMA + TMEM) vs float64 references: every majorness / precision / epilogue variant."""
+"""wgmma GEMM (TMA + wgmma) vs float64 references: every majorness / precision / epilogue variant."""
 import pytest
 
 pytestmark = pytest.mark.gpu
@@ -9,5 +9,5 @@ def test_gemm_tc_all_variants():
 
     rows, txt = run_all()
     bad = [r for r in rows if not r[3]]
-    assert not bad, "tcgen05 GEMM mismatches:\n" + "\n".join(
+    assert not bad, "wgmma GEMM mismatches:\n" + "\n".join(
         f"{n}: err={e:.3e} tol={t:.1e} {d}" for n, e, t, _, d in bad)

@@ -40,4 +40,4 @@ def test_make_cli_goldens_reproduces_the_recorded_reference_run(tmp_path):
 
     assert lines(os.path.join(str(tmp_path), "cli_cfg0_C.txt")) == lines(os.path.join(ROOT, "tests", "golden",
                                                                                      "cli_cfg0_C.txt"))
-    assert os.path.getsize(os.path.join(str(tmp_path), "cli_cfg0_C_ref.pt")) > 1_000_000
+    assert os.path.getsize(os.path.join(str(tmp_path), "cli_cfg0_C_ref.pt")) > 100_000

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Per-task timeline of the persistent MLP-chain kernels (csrc/gemm_chain.cu, dlrm_b200_gemm_chain_set_trace)
-inside real CFG2-shaped training steps.  Writes gpurun_out/<tag>_chain_trace.npz (one [tasks, 8] array per
+inside real CFG2-shaped training steps.  Writes $DLRM_TRACE_DIR (default traces/)/<tag>_chain_trace.npz (one [tasks, 8] array per
 chain: claim, deps ready, last TMA issued, first operands landed, last MMA issued, accumulator ready, epilogue
 done (ns, relative to the first claim), SM id) and prints a per-problem summary.  Run on the GPU box."""
 import os
@@ -69,8 +69,9 @@ def main(tag="trace", B=2048, rows=100_000, T=26):
                       np.median(r[:, 3] - r[:, 1]) / 1e3, np.median(r[:, 4] - r[:, 3]) / 1e3,
                       np.median(r[:, 5] - r[:, 4]) / 1e3, np.median(r[:, 6] - r[:, 5]) / 1e3,
                       r[:, 6].min() / 1e3, r[:, 6].max() / 1e3))
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    np.savez_compressed(os.path.join(ROOT, "gpurun_out", "%s_chain_trace.npz" % tag), **out)
+    out_dir = os.environ.get("DLRM_TRACE_DIR", "traces")
+    os.makedirs(out_dir, exist_ok=True)
+    np.savez_compressed(os.path.join(out_dir, "%s_chain_trace.npz" % tag), **out)
 
 
 if __name__ == "__main__":

@@ -4,7 +4,7 @@ stream, relative to the start of the step -- shows which launches overlap across
 (main / embedding / weight-gradient) and where a stream sits idle.  ncu serialises kernels and flushes
 caches, so it cannot show this; CUDA events on the launching streams can.
 
-    python tools/step_timeline.py [--steps 20] [--pdl 0|1] > gpurun_out/timeline.txt
+    python tools/step_timeline.py [--steps 20] [--pdl 0|1] > timeline.txt
 
 Method: `TimelineEngine` subclasses the product Engine and turns its launch counter (`n_launch`, bumped
 after every C-ABI launch) into a property whose setter records a CUDA event on the current stream,
