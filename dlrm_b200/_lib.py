@@ -28,7 +28,7 @@ class EmbBwdTable(C.Structure):
                 ("indices", C.c_void_p), ("offsets", C.c_void_p), ("nnz", C.c_int64),
                 ("rows", C.c_int64), ("pair_base", C.c_int64), ("ld", C.c_int64), ("mom_stride", C.c_int64),
                 ("use_dy_off", C.c_int64), ("dy_off", C.c_int64), ("row_lo", C.c_int64), ("row_n", C.c_int64),
-                ("head_stride", C.c_int64)]
+                ("head_stride", C.c_int64), ("mark", C.c_void_p)]
 
 
 class EmbRemoteTable(C.Structure):

@@ -26,7 +26,7 @@ enum Tunable {
   TUNE_HEAD_ROWS = 6,           // samples per CTA in the fused head (16 or 32; 0 = default)
   TUNE_INTERACT_BWD_COLS = 7,   // 1 = one column per thread (first kernel), else float2 columns
   TUNE_PDL = 8,                 // programmatic dependent launch on the dense chain: 0/1 = on, 2 = off
-  TUNE_UPD_LEAN = 10,           // embedding update, dim <= 128: 0 = default lean variant, 1/3..7 = variants (emb_bwd.cu), 2 = general kernel
+  TUNE_UPD_LEAN = 10,           // embedding update, dim <= 128: 2 = the general kernel instead of the lean one
   TUNE_UPD_DEBUG = 11,          // timing experiments on the update kernel (see EmbBwdParams::debug); 0 = off
   TUNE_CHAIN_ORDER = 9,         // gemm_chain task order: 0/1 = layer by layer, 2 = m-tile major across layers
   TUNE_COUNT = 16

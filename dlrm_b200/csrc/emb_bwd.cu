@@ -10,15 +10,23 @@
 //   link   : every occurrence `pos` of a row threads itself onto a per-row list with one
 //            atomicExch on head[row] (int32 per table row, zero between steps):
 //                link[pos] = { previous head, bag of pos };  head[row] = pos + 1
-//            Depends on the indices only -> can overlap the forward pass.
-//   update : one warp per bag.  Occurrence `pos` owns its row iff head[row] == pos + 1 (the
-//            last arrival).  The owner walks the list, sorts the members by position when there
-//            are <= 32 (deterministic sum in ascending position == grad.coalesce() order; a longer list
-//            takes the order-independent fixed-point sum of list_sum_exact), adds
-//            their dY rows, applies the optimizer to the 512-byte weight row in registers and
-//            resets head[row] = 0.  Non-owners do nothing.  Rows without duplicates (the common
-//            case at 1e6-row tables) never touch link[] beyond their own entry and reuse the
-//            bag's own dY row, which is loaded once per bag.
+//            and, when the previous head p + 1 is not 0, marks occurrence p as superseded:
+//                mark[p] = 1     (one byte per position, zero between steps)
+//            Every position is superseded by at most one successor, so a plain store does; only
+//            duplicate occurrences write, and the array (1 byte x occurrences) stays in L2.
+//            Depends on the indices only -> can overlap the forward pass (or ride in the gather).
+//   update : a warp takes 32 consecutive positions and reads index, link entry and mark of each
+//            (coalesced), clearing the marks it read.  Occurrence `pos` owns its row iff it is not
+//            marked (the last arrival): ownership is decided without touching the table.  The owner
+//            issues the loads of the weight row and of the row's accumulator together (with the
+//            interleaved layout the accumulator and the list head sit right behind the row, in the
+//            same DRAM page), walks the list when there is one, sorts the members by position when
+//            there are <= 32 (deterministic sum in ascending position == grad.coalesce() order; a
+//            longer list takes the order-independent fixed-point sum of list_sum_exact), adds their
+//            dY rows, applies the optimizer in registers and stores the row, the accumulator and
+//            head[row] = 0 together.  Two random DRAM accesses per updated row: row + words in,
+//            row + words out.  Non-owners do nothing.  Rows without duplicates (the common case at
+//            1e6-row tables) never touch link[] beyond their own entry.
 #include "common.cuh"
 
 namespace dlrm {
@@ -83,16 +91,29 @@ __device__ __forceinline__ void list_sum_exact(const int2* link, int nxt, int se
   ListWalk w{link, nxt, self_bag, true, 0u, 0ull};
   ListWalk resume = w;
   int n = 0;
+  // members of a chunk are visited LB at a time: their dY rows are all loaded before the first is used
+  constexpr int LB = N <= 4 ? 4 : 1;
+  auto visit = [&](int bag, int cnt, auto&& use) {
+    for (int q0 = 0; q0 < cnt; q0 += LB) {
+      float t[LB][N];
+#pragma unroll
+      for (int u = 0; u < LB; ++u) {
+        const int b = __shfl_sync(0xffffffffu, bag, (q0 + u) & 31);
+        if (q0 + u < cnt) load(b, t[u]);
+      }
+#pragma unroll
+      for (int u = 0; u < LB; ++u)
+        if (q0 + u < cnt) use(t[u]);
+    }
+  };
   for (int c = 0; !w.done(); ++c) {                    // pass 1: column maxima
     int bag = 0;
     const int cnt = w.chunk(lane, bag);
     if (c < LS_KEEP) { keep[c] = bag; cnt_keep[c] = cnt; resume = w; }
-    for (int q = 0; q < cnt; ++q) {
-      float t[N];
-      load(__shfl_sync(0xffffffffu, bag, q), t);
+    visit(bag, cnt, [&](const float (&t)[N]) {
 #pragma unroll
       for (int j = 0; j < N; ++j) mx[j] = fmaxf(mx[j], fabsf(t[j]));
-    }
+    });
     n += cnt;
   }
   const int L = 32 - __clz(n);                          // n < 2^L
@@ -108,12 +129,10 @@ __device__ __forceinline__ void list_sum_exact(const int2* link, int nxt, int se
     f[j] = 0.f;
   }
   auto add_chunk = [&](int bag, int cnt) {
-    for (int q = 0; q < cnt; ++q) {
-      float t[N];
-      load(__shfl_sync(0xffffffffu, bag, q), t);
+    visit(bag, cnt, [&](const float (&t)[N]) {
 #pragma unroll
       for (int j = 0; j < N; ++j) { s[j] += (long long)((double)t[j] * sc[j]); f[j] += t[j]; }
-    }
+    });
   };
 #pragma unroll
   for (int c = 0; c < LS_KEEP; ++c)                    // pass 2: the kept chunks, then the rest of the list
@@ -142,6 +161,7 @@ struct EmbBwdTable {
   long long rows;        // rows of the whole table
   long long row_lo;      // this shard stores rows [row_lo, row_lo + row_n) at local index (row - row_lo);
   long long row_n;       //   occurrences of other rows belong to another shard and are ignored
+  unsigned char* mark;   // superseded marks, indexed like link[]
 };
 
 struct EmbBwdParams {
@@ -205,6 +225,7 @@ __global__ void __launch_bounds__(256) emb_link_kernel(const __grid_constant__ E
     const bool mine = tb.head != nullptr && (unsigned long long)r < (unsigned long long)tb.row_n;
     const int prev = mine ? atomicExch(tb.head + r * tb.hs, (int)(pos + 1)) : 0;
     P.link[pos] = make_int2(prev, (int)lo);
+    if (prev) tb.mark[prev - 1] = 1;          // that occurrence is no longer the last one of its row
   }
 }
 
@@ -311,7 +332,9 @@ __global__ void __launch_bounds__(256) emb_link_suspects_kernel(const __grid_con
     const long long pos = suspects[i];
     const EmbBwdTable& tb = P.t[table_of(bound, num_tables, pos)];
     const long long r = static_cast<const idx_t*>(tb.idx)[pos - tb.pair_base];
-    P.link[pos].x = atomicExch(tb.head + r * tb.hs, (int)(pos + 1));
+    const int prev = atomicExch(tb.head + r * tb.hs, (int)(pos + 1));
+    P.link[pos].x = prev;
+    if (prev) tb.mark[prev - 1] = 1;
   }
 }
 
@@ -365,24 +388,24 @@ __global__ void __launch_bounds__(256, NV == 1 ? 3 : 1) emb_update_kernel(const 
     const int k = table_of(bound, num_tables, pos < total ? pos : first);
     const bool valid = pos < total && pos < tend[k];
     long long my_r = 0;
-    int my_head = 0;
     int2 my_link = make_int2(0, 0);
     bool my_susp = true;
-    bool mine = false;
+    bool owner = false;
     if (valid) {
       const EmbBwdTable& tb = P.t[k];
       my_r = (long long)static_cast<const idx_t*>(tb.idx)[pos - tb.pair_base] - tb.row_lo;
       // rows of another shard, and tables updated by the small-table path (head == null), are not ours
-      mine = tb.head != nullptr && (unsigned long long)my_r < (unsigned long long)tb.row_n;
-      if (mine) {
+      if (tb.head != nullptr && (unsigned long long)my_r < (unsigned long long)tb.row_n) {
         my_link = P.link[pos];
+        const unsigned char superseded = tb.mark[pos];
+        if (superseded) tb.mark[pos] = 0;
+        owner = !superseded;
+        // an unflagged occurrence is the only one of its row (never linked, never marked): head[] is never touched
         if (P.flags) my_susp = P.flags[pos] != 0;
-        // an unflagged occurrence is the only one of its row: it owns the row, head[] is never touched
-        my_head = my_susp ? tb.head[my_r * tb.hs] : (int)(pos + 1);
         if (!my_susp) my_link.x = 0;
       }
     }
-    const unsigned owners = __ballot_sync(0xffffffffu, mine && my_head == (int)(pos + 1));
+    const unsigned owners = __ballot_sync(0xffffffffu, owner);
     const unsigned susp_mask = __ballot_sync(0xffffffffu, my_susp);
     for (int u0 = 0; u0 < 32; u0 += PF) {
       if (((owners >> u0) & ((1u << PF) - 1u)) == 0u) continue;
@@ -501,18 +524,21 @@ __global__ void __launch_bounds__(256, NV == 1 ? 3 : 1) emb_update_kernel(const 
 // per step and GPU) that makes the update instruction-bound instead of bound by random DRAM accesses.  Here
 //   * the per-table fields live in shared memory, a 32-position window takes its table from lane 0 unless
 //     the window straddles a table boundary;
-//   * every lane resolves ITS occurrence once into two pointers (weight row, gradient row) + the list head;
-//     owners are compacted with ballot/ffs and processed PF at a time: 2 pointer broadcasts + 2 row loads
-//     each, all issued before the first use;
+//   * every lane resolves ITS occurrence once (ownership from the coalesced mark, no table access) into
+//     pointers to the weight row, gradient row, accumulator and list head; owners are compacted with
+//     ballot/ffs and processed PF at a time: 2 pointer broadcasts + 2 row loads each, the owning lane loads
+//     the accumulator, all issued before the first use;
 //   * the row update is w += (-lr / (sqrt(m) + eps)) * g -- one reciprocal per row instead of a division per
 //     element (differs from g / std by <= 1 ulp per element; the tests' tolerance is 2e-5 relative);
-//   * the owning lane itself stores the accumulator and clears the list head (no pointer broadcast);
+//   * the owning lane itself stores the accumulator and clears the list head with the row's store (no
+//     pointer broadcast);
 //   * rows with duplicates (rare at large tables) take an out-of-line path.
 // ---------------------------------------------------------------------------------------------
 struct UpdTableS {
   float* w;
   float* mom;
   int* head;
+  unsigned char* mark;
   const void* idx;
   long long pair_base, ld, mom_stride, hs, dy_off, row_lo, row_n;
 };
@@ -548,38 +574,33 @@ __device__ __noinline__ float4 upd_sum_duplicates(const EmbBwdParams& P, int nxt
   if (nxt != 0) return upd_sum_long(P, nxt0, self_bag, dy_off, col_ok);
   int rank = 0;
   for (int i = 0; i < cnt; ++i) rank += (__shfl_sync(0xffffffffu, mpos, i) < mpos) ? 1 : 0;
-  for (int q = 0; q < cnt; ++q) {
-    const unsigned who = __ballot_sync(0xffffffffu, lane < cnt && rank == q);
-    const int bag = __shfl_sync(0xffffffffu, mbag, __ffs(who) - 1);
-    if (col_ok) {
-      const float4 t = *reinterpret_cast<const float4*>(dy_row(P, bag) + dy_off + lane * 4);
-      g.x += t.x; g.y += t.y; g.z += t.z; g.w += t.w;
+  // the dY rows of DUP_BATCH members are loaded before any of them is added (one round trip per batch instead of
+  // one per member); the adds keep the ascending-position order
+  constexpr int DUP_BATCH = 4;
+  for (int q0 = 0; q0 < cnt; q0 += DUP_BATCH) {
+    float4 t[DUP_BATCH];
+#pragma unroll
+    for (int u = 0; u < DUP_BATCH; ++u) {
+      const unsigned who = __ballot_sync(0xffffffffu, lane < cnt && rank == q0 + u);
+      const int bag = __shfl_sync(0xffffffffu, mbag, who ? __ffs(who) - 1 : 0);
+      t[u] = (who && col_ok) ? *reinterpret_cast<const float4*>(dy_row(P, bag) + dy_off + lane * 4)
+                             : make_float4(0.f, 0.f, 0.f, 0.f);
     }
+#pragma unroll
+    for (int u = 0; u < DUP_BATCH; ++u)
+      if (q0 + u < cnt && col_ok) { g.x += t[u].x; g.y += t[u].y; g.z += t[u].z; g.w += t[u].w; }
   }
   return g;
 }
 
-// One window (32 consecutive occurrence positions, one per lane) in flight between the stages of the update:
-// stage 0 reads the index and the list entry (coalesced), stage 1 the row's list head and accumulator (one random
-// sector), stage 2 updates the rows this window owns.  PIPE: stage 0 of window w+2 and stage 1 of window w+1 are
-// issued BEFORE stage 2 of window w, so their two dependent round trips (a random access over > 100 GB of tables
-// takes microseconds under load) hide behind the row traffic instead of preceding it.
-struct UpdWin {
-  int k;        // table of the lane's position
-  int r;        // row inside the shard, -1: not this kernel's (padding, another shard, a gap between tables)
-  int2 lk;      // list entry of the position: (previous occurrence + 1, bag)
-  int hd;       // the row's list head
-  float m;      // the row's accumulator
-};
-
-template <typename idx_t, int PF, int MINB, bool PIPE>      // PF: row PAIRS in flight per warp
+template <typename idx_t, int PF, int MINB>      // PF: row PAIRS in flight per warp
 __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid_constant__ EmbBwdParams P, int num_tables,
                                                                     long long total_hint) {
   __shared__ long long bound[DLRM_B200_MAX_TABLES_PER_CALL + 1], tend[DLRM_B200_MAX_TABLES_PER_CALL + 1];
   __shared__ UpdTableS ts[DLRM_B200_MAX_TABLES_PER_CALL];
   for (int k = threadIdx.x; k < num_tables; k += blockDim.x) {
     UpdTableS t;
-    t.w = P.t[k].w; t.mom = P.t[k].mom; t.head = P.t[k].head; t.idx = P.t[k].idx;
+    t.w = P.t[k].w; t.mom = P.t[k].mom; t.head = P.t[k].head; t.mark = P.t[k].mark; t.idx = P.t[k].idx;
     t.pair_base = P.t[k].pair_base; t.ld = P.t[k].ld; t.mom_stride = P.t[k].mom_stride; t.hs = P.t[k].hs;
     t.dy_off = P.t[k].dy_off; t.row_lo = P.t[k].row_lo; t.row_n = P.t[k].row_n;
     ts[k] = t;
@@ -601,66 +622,37 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
   const bool adagrad = P.optimizer == DLRM_OPT_RWSADAGRAD;
   const int dbg = P.debug;
 
-  auto stage0 = [&](long long base, UpdWin& w) {
-    w.r = -1;
-    w.k = 0;
-    w.lk = make_int2(0, 0);
-    if (base >= total) return;
+  for (long long base = first + warp0 * 32; base < total; base += wstep) {
+    // index, list entry and mark of the 32 positions of the window: coalesced, and all that ownership needs
     const long long pos = base + lane;
     // table of this window: lane 0's, unless the window crosses into the next table
     int k = table_of(bound, num_tables, base);
     if (base + 31 >= bound[k + 1]) k = table_of(bound, num_tables, pos < total ? pos : base);
-    w.k = k;
     const UpdTableS& tb = ts[k];
+    int r = 0;
+    int2 lk = make_int2(0, 0);
+    bool owner = false;
     if (pos < total && pos < tend[k] && tb.head != nullptr) {   // positions between two tables of the call are not ours
-      const long long r = (long long)static_cast<const idx_t*>(tb.idx)[pos - tb.pair_base] - tb.row_lo;
-      w.lk = P.link[pos];
-      if ((unsigned long long)r < (unsigned long long)tb.row_n) w.r = (int)r;
+      const long long rr = (long long)static_cast<const idx_t*>(tb.idx)[pos - tb.pair_base] - tb.row_lo;
+      lk = P.link[pos];
+      const unsigned char superseded = tb.mark[pos];
+      if (superseded) tb.mark[pos] = 0;
+      // the last occurrence to arrive (never superseded) owns the row; rows of another shard are not ours
+      owner = (unsigned long long)rr < (unsigned long long)tb.row_n && !superseded;
+      r = (int)rr;
     }
-  };
-  auto stage1 = [&](UpdWin& w) {
-    w.hd = 0;
-    w.m = 0.f;
-    if (w.r >= 0) {
-      const UpdTableS& tb = ts[w.k];
-      w.hd = tb.head[(long long)w.r * tb.hs];
-      if (adagrad) w.m = tb.mom[(long long)w.r * tb.mom_stride];
-    }
-  };
-
-  long long base = first + warp0 * 32;
-  UpdWin w1, w2;                 // w1: stage 1 issued; w2: stage 0 issued
-  if (PIPE) {
-    stage0(base, w1);
-    stage1(w1);
-    stage0(base + wstep, w2);
-  }
-  for (; base < total; base += wstep) {
-    UpdWin w;
-    if (PIPE) {
-      w = w1;
-      w1 = w2;
-      stage1(w1);                              // head + accumulator of the next window
-      stage0(base + 2 * wstep, w2);            // index + list entry of the one after
-    } else {
-      stage0(base, w);
-      stage1(w);
-    }
-    const long long pos = base + lane;
-    const UpdTableS& tb = ts[w.k];
-    const bool owner = w.r >= 0 && w.hd == (int)(pos + 1);      // the last occurrence to arrive owns the row
-    const int nxt = owner ? w.lk.x : 0, bag = w.lk.y;
-    float* wptr = owner ? tb.w + (long long)w.r * tb.ld : nullptr;
+    const int nxt = owner ? lk.x : 0, bag = lk.y;
+    float* wptr = owner ? tb.w + (long long)r * tb.ld : nullptr;
     const float* gptr = owner ? dy_row(P, bag) + tb.dy_off : nullptr;
-    float* mptr = (owner && adagrad) ? tb.mom + (long long)w.r * tb.mom_stride : nullptr;
-    int* hptr = owner ? tb.head + (long long)w.r * tb.hs : nullptr;
-    const float m_old = owner ? w.m : 0.f;
+    float* mptr = (owner && adagrad) ? tb.mom + (long long)r * tb.mom_stride : nullptr;
+    int* hptr = owner ? tb.head + (long long)r * tb.hs : nullptr;
     unsigned simple = __ballot_sync(0xffffffffu, owner && nxt == 0);
     unsigned dups = __ballot_sync(0xffffffffu, owner && nxt != 0);
 
     // ---------------------------------------------------------------- rows without duplicates, two per step
     while (simple) {
       float4 wv[PF][2], gv[PF][2];
+      float mv[PF];
       int sa[PF], sb[PF];
 #pragma unroll
       for (int u = 0; u < PF; ++u) {
@@ -678,6 +670,8 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
         wv[u][1] = (s_ >= 0 && c1_ok && ldw) ? *reinterpret_cast<const float4*>(wp + 4) : z;
         gv[u][0] = (s_ >= 0 && c0_ok && ldg) ? *reinterpret_cast<const float4*>(gp) : z;
         gv[u][1] = (s_ >= 0 && c1_ok && ldg) ? *reinterpret_cast<const float4*>(gp + 4) : z;
+        // the owning lanes load their accumulators in the same batch as the rows
+        mv[u] = (adagrad && (lane == sa[u] || lane == sb[u])) ? *mptr : 0.f;
       }
 #pragma unroll
       for (int u = 0; u < PF; ++u) {
@@ -691,7 +685,7 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
           sq = fmaf(g1.x, g1.x, fmaf(g1.y, g1.y, fmaf(g1.z, g1.z, fmaf(g1.w, g1.w, sq))));
 #pragma unroll
           for (int o = 8; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);     // within the half
-          const float m_new = __shfl_sync(0xffffffffu, m_old, sc) + sq * inv_d;
+          const float m_new = __shfl_sync(0xffffffffu, mv[u], sc) + sq * inv_d;
           scale = nlr / (sqrtf(m_new) + P.eps);
           const float mA = __shfl_sync(0xffffffffu, m_new, 0), mB = __shfl_sync(0xffffffffu, m_new, 16);
           if (lane == sa[u] && !(dbg & 4)) *mptr = mA;               // the owning lanes store their accumulators
@@ -718,6 +712,7 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
       const long long dyo = __shfl_sync(0xffffffffu, tb.dy_off, s_);       // the OWNER's table (windows may straddle)
       float* wp = reinterpret_cast<float*>(__shfl_sync(0xffffffffu, (unsigned long long)wptr, s_));
       float4 w = col_ok ? *reinterpret_cast<const float4*>(wp + lane * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
+      const float m_old = (adagrad && lane == s_) ? *mptr : 0.f;
       const float4 g = upd_sum_duplicates(P, nx, (int)(base + s_), sbg, dyo, lane, col_ok);
       float scale = nlr;
       if (adagrad) {
@@ -748,6 +743,8 @@ static int fill_params(EmbBwdParams& P, const dlrm_emb_bwd_table_t* tables, int 
     P.t[k].w = tables[k].weight;
     P.t[k].mom = tables[k].momentum;
     P.t[k].head = tables[k].head;
+    P.t[k].mark = tables[k].mark;
+    if (tables[k].head && !tables[k].mark) return set_error("%s: table %d: head without a mark array", who, k);
     P.t[k].idx = tables[k].indices;
     P.t[k].off = tables[k].offsets;
     P.t[k].nnz = tables[k].nnz;
@@ -869,30 +866,14 @@ static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, i
     return 0;                                                                                              \
   } while (0)
   if (vec && dim <= 128 && !P.flags && get_tunable(TUNE_UPD_LEAN) != 2) {
-    // 3 CTAs of 256 threads per SM (<= 85 registers, no spills)
     long long gl = (total / 32 + block / 32) / (block / 32);
     if (gl > (long long)sms * 3) gl = (long long)sms * 3;
     if (gl < 1) gl = 1;
-    // TUNE_UPD_LEAN (variants compared with tools/upd_variants.py): 0/3 (default) = 2 row pairs in flight per warp,
-    // 3 CTAs/SM; 5 = 3 pairs, 3 CTAs/SM; 4 = 2 pairs, 3 CTAs/SM, software-pipelined windows; 1 = pipelined, 3 pairs,
-    // 2 CTAs/SM; 6 / 7 = 4 pairs, 2 CTAs/SM, pipelined / not (2 = the general kernel).  The kernel is bound by the
-    // RATE of random accesses (list head + accumulator, row read, row write), not by the latency of any one of them.
-    int var = (int)get_tunable(TUNE_UPD_LEAN);
-    if (var == 0) var = 3;
-    const int per_sm = (var == 1 || var == 6 || var == 7) ? 2 : 3;
-    if (gl > (long long)sms * per_sm) gl = (long long)sms * per_sm;
-#define LEAN(IT)                                                                                                   \
-    do {                                                                                                            \
-      if (var == 5) emb_update_lean_kernel<IT, 3, 3, false><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);  \
-      else if (var == 4) emb_update_lean_kernel<IT, 2, 3, true><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);   \
-      else if (var == 6) emb_update_lean_kernel<IT, 4, 2, true><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);   \
-      else if (var == 7) emb_update_lean_kernel<IT, 4, 2, false><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);  \
-      else if (var == 1) emb_update_lean_kernel<IT, 3, 2, true><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);   \
-      else emb_update_lean_kernel<IT, 2, 3, false><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);                \
-    } while (0)
-    if (idx_bytes == 8) LEAN(long long);
-    else LEAN(int);
-#undef LEAN
+    // 3 CTAs of 256 threads per SM (<= 85 registers), 2 row pairs in flight per warp: on H100 (cfg3) 3 pairs /
+    // 3 CTAs and 4 pairs / 2 CTAs per SM were measured no faster and 8 % slower.  The kernel is bound by the RATE of random accesses
+    // (row + accumulator read, row + accumulator + head write), not by the latency of any one of them.
+    if (idx_bytes == 8) emb_update_lean_kernel<long long, 2, 3><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);
+    else emb_update_lean_kernel<int, 2, 3><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);
     DLRM_CHECK_LAUNCH("emb_update_lean_kernel");
     return 0;
   }

@@ -23,6 +23,7 @@ struct EmbFwdTable {
   long long hs;         // elements between the list heads of consecutive rows (1, or the row stride when the
                         // head lives inside the row's own DRAM page: [weights | accumulator | head | pad])
   long long pair_base;  // training: first slot of this table in link[]
+  unsigned char* mark;  // training: superseded marks, indexed like link[] (see emb_bwd.cu)
   long long ld;         // row stride in floats
   long long out_off;    // pooled row of bag b goes to out_row(b) [+ b_local * out_stride] + out_off
   long long out_stride; // elements between consecutive samples of THIS table's output
@@ -187,8 +188,10 @@ __global__ void __launch_bounds__(256, (G == 32 && NV == 1) ? 4 : 1) emb_fwd_vec
             }
           }
         }
-        if (link_tb && j0 + gl < end)
+        if (link_tb && j0 + gl < end) {
           P.link[tb.pair_base + j0 + gl] = make_int2(my_prev, (int)(b0 + s));
+          if (my_prev) tb.mark[my_prev - 1] = 1;   // that occurrence is no longer the last one of its row
+        }
       }
       float* op = out_ptr(P, tb, b0 + s) + gl * 4;
 #pragma unroll
@@ -237,8 +240,11 @@ __global__ void __launch_bounds__(256) emb_fwd_shard_kernel(const __grid_constan
       const long long lr = rg - tb.row_lo;
       const bool mine = valid && (unsigned long long)lr < (unsigned long long)tb.row_n;
       if (valid && !mine && (unsigned long long)rg >= (unsigned long long)tb.rows) flag_bad_index(P);
-      if (link_tb && mine)      // occurrences of other shards' rows are never looked at by the update
-        P.link[tb.pair_base + j0 + gl] = make_int2(note_occurrence(P, tb, lr, j0 + gl), (int)b);
+      if (link_tb && mine) {    // occurrences of other shards' rows are never looked at by the update
+        const int prev = note_occurrence(P, tb, lr, j0 + gl);
+        P.link[tb.pair_base + j0 + gl] = make_int2(prev, (int)b);
+        if (prev) tb.mark[prev - 1] = 1;
+      }
       unsigned live = (__ballot_sync(gmask, mine) >> (grp * G)) & gbits;
       while (live) {
         float4 val[U][NV];
@@ -383,7 +389,11 @@ __global__ void emb_fwd_scalar_kernel(const __grid_constant__ EmbFwdParams P) {
     const long long r = rg - tb.row_lo;
     const bool mine = (unsigned long long)r < (unsigned long long)tb.row_n;
     if (!mine && (unsigned long long)rg >= (unsigned long long)tb.rows && d == 0) flag_bad_index(P);
-    if (LINK && tb.head && d == 0) P.link[tb.pair_base + j] = make_int2(mine ? note_occurrence(P, tb, r, j) : 0, (int)b);
+    if (LINK && tb.head && d == 0) {
+      const int prev = mine ? note_occurrence(P, tb, r, j) : 0;
+      P.link[tb.pair_base + j] = make_int2(prev, (int)b);
+      if (prev) tb.mark[prev - 1] = 1;
+    }
     if (!mine) continue;
     const float x = tb.w[r * tb.ld + d];
     acc = WEIGHTED ? fmaf(tb.rw[r], x, acc) : acc + x;
@@ -470,6 +480,8 @@ static int emb_fwd_impl(const dlrm_emb_fwd_table_t* tables, const dlrm_emb_bwd_t
     P.t[k].head = train ? train[k].head : nullptr;   // train[k].head == NULL: this table is not linked
     P.t[k].hs = (train && train[k].head_stride > 0) ? train[k].head_stride : 1;
     P.t[k].pair_base = train ? train[k].pair_base : 0;
+    P.t[k].mark = train ? train[k].mark : nullptr;
+    if (P.t[k].head && !P.t[k].mark) return set_error("emb_bag_fwd_train: table %d: head without a mark array", k);
     // per-table output routing (0 = the call-level layout out[b, k, :])
     P.t[k].out_stride = tables[k].out_stride > 0 ? tables[k].out_stride : out_stride_sample;
     P.t[k].out_off = tables[k].out_stride > 0 ? tables[k].out_off : (int64_t)k * out_stride_table;

@@ -14,6 +14,7 @@ HBM layout (fp32 unless noted)
   tables   [sum_k rows_k, D]   one allocation; table k = rows [row_base_k, row_base_k + rows_k)
   momentum [sum_k rows_k]      RWSAdagrad row-wise accumulator (optim/rwsadagrad.py:91-95)
   head     [sum_k rows_k] i32  per-row list heads for the sort-free coalesce (zero between steps)
+  mark     [nnz] u8            per-occurrence superseded marks beside link[] (zero between steps)
   dense    [P]                 bot W0,b0,W1,b1,... top W0,b0,...  (+ grad arena, + Adagrad sums)
   T        [B, F, D]           interaction operand: feature 0 <- last bottom-MLP epilogue,
                                feature 1+k <- gather of table k (torch.cat K3 eliminated)
@@ -238,10 +239,11 @@ class Engine:
         self.loss_buf = torch.zeros(1, dtype=f32, device=dev)
         self.scratch = torch.zeros(1024, dtype=f32, device=dev)
         self.link = None  # int32 [2 * nnz capacity]
+        self.mark = None  # uint8 [nnz capacity]: occurrence superseded by a later one of its row (zero between steps)
         self.dedup, self._filtered = None, False
-        # Optional duplicate filter for the training gather / update (dlrm_emb_dedup_t).  It removes the list-head
-        # traffic from the update but adds a memset + two small launches to the gather side, while the row
-        # read-modify-write and the accumulator accesses dominate the update; OFF by default.
+        # Optional duplicate filter for the training gather / update (dlrm_emb_dedup_t).  It removes the gather's
+        # list-head atomics but adds a memset + two small launches to the gather side and runs the general update
+        # kernel instead of the lean one; OFF by default.
         self.use_filter = False
 
     def is_small(self, j: int) -> bool:
@@ -328,6 +330,7 @@ class Engine:
         if self.link is None or self.link.numel() < 2 * nnz_total:
             cap = max(2 * nnz_total, 1024)
             self.link = torch.empty(cap, dtype=torch.int32, device=self.device)
+            self.mark = torch.zeros(cap // 2, dtype=torch.uint8, device=self.device)
             # duplicate filter (see include/dlrm_b200.h, dlrm_emb_dedup_t): ~8 hashed counters per occurrence
             n = max(nnz_total, 512)
             log2 = max(16, int(np.ceil(np.log2(8 * n))))
@@ -448,6 +451,7 @@ class Engine:
                 d.head, d.head_stride = d.weight + (self.D + 1) * 4, self.ldw
             else:
                 d.head, d.head_stride = self._head_sep.data_ptr() + int(self.row_base[k]) * 4, 1
+            d.mark = self.mark.data_ptr() if self.mark is not None else None
             d.indices = sp.indices[k].data_ptr() if sp.indices[k].numel() else 0
             d.offsets = sp.offsets[k].data_ptr()
             d.nnz = sp.indices[k].numel()

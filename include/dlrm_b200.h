@@ -95,9 +95,12 @@ int dlrm_b200_emb_bag_fwd(const dlrm_emb_fwd_table_t* tables /*[host]*/, int num
  *
  * Step 1, dlrm_b200_emb_bwd_link: depends on the indices only (can run on a side stream
  * during the forward pass).  Threads every (table,row) occurrence of the batch onto a
- * per-row list: prev = atomicExch(&head[row], pos+1); next[pos] = prev.  `head` is an int32
- * array over all rows of the table, zero on entry and zero again after step 2.
- * Step 2, dlrm_b200_emb_bwd_update: one warp per bag; the list head (= unique owner of a row)
+ * per-row list: prev = atomicExch(&head[row], pos+1); next[pos] = prev; and, when prev != 0,
+ * mark[prev-1] = 1 (that occurrence is no longer the last one of its row).  `head` is an int32
+ * array over all rows of the table, `mark` a byte per occurrence position; both are zero on
+ * entry and zero again after step 2.
+ * Step 2, dlrm_b200_emb_bwd_update: the last occurrence of a row (the unmarked one) owns it,
+ * known from the coalesced mark[] without touching the table; it
  * sums dY over the row's occurrences: up to 32 in ascending position (== grad.coalesce()), more
  * with an order-independent fixed-point sum (the same result on every run), then
  *   RWSAdagrad: momentum[row] += mean_d(g^2); W[row] -= lr * g / (sqrt(momentum[row]) + eps)
@@ -127,18 +130,24 @@ typedef struct {
   int64_t row_lo, row_n;
   /* elements between consecutive rows' list heads; 0 = 1.  head = (int32*)weight + dim + 1 with head_stride = ld
    * (and momentum = weight + dim, mom_stride = ld, ld = dim + 4) keeps BOTH per-row words inside the row's own
-   * DRAM page: the update is bound by the RATE of random DRAM accesses (~10 G/s measured: the gather's 512-byte
-   * rows and the update's 4-byte words cost the same), so 6 accesses per occurrence become 2-3. */
+   * DRAM page.  The update is bound by the RATE of random DRAM accesses (the gather's 512-byte rows and the
+   * update's 4-byte words cost about the same), and with the marks below the owner of a row reads the two words
+   * in the same batch as the row and writes them with the row: two random accesses per updated row (row +
+   * words in, row + words out) instead of four. */
   int64_t head_stride;
+  /* [positions] superseded marks, indexed like next[] (pair_base + j): mark[p] = 1 once a later occurrence of
+   * the same row was linked.  Zero-initialised scratch, all zero between steps (the update clears what the
+   * link set).  Required whenever head != NULL. */
+  uint8_t* mark;
 } dlrm_emb_bwd_table_t;
 
 /* Optional duplicate filter (dlrm_emb_dedup_t): at 1e6-row tables almost every row of a batch is
- * touched once, and the 4-byte random accesses to head[] cost as much HBM time as the 512-byte rows.
+ * touched once, and the gather's atomicExch on head[] is a random 4-byte access per occurrence.
  * With a filter the training gather only bumps a counter in an L2-sized hashed array
  * (fire-and-forget RED), dlrm_b200_emb_bwd_classify() -- right after the gather, while the
  * counters are L2-hot -- marks the occurrences whose counter is > 1 as suspects (hash collisions
- * only add false suspects) and threads ONLY those onto the per-row lists; the update kernel then
- * treats unflagged occurrences as sole owners of their row without touching head[] or link[].x.
+ * only add false suspects) and threads ONLY those onto the per-row lists; the update then treats
+ * unflagged occurrences as sole owners of their row and leaves their head[] and link[].x alone.
  *   filter   : uint32 [2^log2_size + 1], zeroed by the caller before every training gather
  *              (the last element is the suspect counter)
  *   flags    : uint8  [nnz capacity]   suspects : int32 [nnz capacity]

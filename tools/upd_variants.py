@@ -1,5 +1,5 @@
 """Time the embedding update (and the training gather) of one workload for several kernel variants in ONE process:
-   python tools/upd_variants.py [cfg3|cfg2] 1,5,4,6,7,3
+   python tools/upd_variants.py [cfg3|cfg2] 0,2        (0 = the lean kernel, 2 = the general one)
 prints one line per TUNE_UPD_LEAN value (median microseconds of the update launch group between CUDA events)."""
 import os
 import sys
@@ -15,7 +15,7 @@ from dlrm_b200 import _lib, dist as ddist, placement as P  # noqa: E402
 from dlrm_b200.data import DeviceBatch  # noqa: E402
 
 name = sys.argv[1] if len(sys.argv) > 1 else "cfg3"
-variants = [int(v) for v in (sys.argv[2] if len(sys.argv) > 2 else "1,5,4,6,7,3").split(",")]
+variants = [int(v) for v in (sys.argv[2] if len(sys.argv) > 2 else "0,2").split(",")]
 os.environ.update(RANK="0", WORLD_SIZE="1", LOCAL_RANK="0", MASTER_ADDR="127.0.0.1", MASTER_PORT=str(bench._free_port()))
 ddist.init_distributed("nccl")
 dev = "cuda:0"
