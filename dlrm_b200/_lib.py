@@ -13,6 +13,7 @@ ACT_NONE, ACT_RELU, ACT_SIGMOID = 0, 1, 2
 LOSS_MSE, LOSS_BCE, LOSS_WBCE = 0, 1, 2
 OPT_SGD, OPT_RWSADAGRAD = 0, 1
 GEMM_SIMT_FP32, GEMM_TC_BF16X3, GEMM_TC_BF16 = 0, 1, 2
+DTYPE_F32, DTYPE_F16 = 0, 1
 TUNE = dict(emb_bags_per_group=0, emb_unroll=1, emb_block=2, upd_block=3, gemm_splitk=4, gemm_smem_kb=5,
             head_rows=6, interact_bwd_cols=7, pdl=8, chain_order=9, upd_lean=10, upd_debug=11)
 
@@ -20,7 +21,8 @@ TUNE = dict(emb_bags_per_group=0, emb_unroll=1, emb_block=2, upd_block=3, gemm_s
 class EmbFwdTable(C.Structure):
     _fields_ = [("weight", C.c_void_p), ("indices", C.c_void_p), ("offsets", C.c_void_p),
                 ("row_weights", C.c_void_p), ("nnz", C.c_int64), ("rows", C.c_int64), ("ld", C.c_int64),
-                ("out_off", C.c_int64), ("out_stride", C.c_int64), ("row_lo", C.c_int64), ("row_n", C.c_int64)]
+                ("out_off", C.c_int64), ("out_stride", C.c_int64), ("row_lo", C.c_int64), ("row_n", C.c_int64),
+                ("weight_dtype", C.c_int32)]
 
 
 class EmbBwdTable(C.Structure):
@@ -28,13 +30,14 @@ class EmbBwdTable(C.Structure):
                 ("indices", C.c_void_p), ("offsets", C.c_void_p), ("nnz", C.c_int64),
                 ("rows", C.c_int64), ("pair_base", C.c_int64), ("ld", C.c_int64), ("mom_stride", C.c_int64),
                 ("use_dy_off", C.c_int64), ("dy_off", C.c_int64), ("row_lo", C.c_int64), ("row_n", C.c_int64),
-                ("head_stride", C.c_int64), ("mark", C.c_void_p)]
+                ("head_stride", C.c_int64), ("mark", C.c_void_p), ("weight_dtype", C.c_int32),
+                ("round_key", C.c_uint64)]
 
 
 class EmbRemoteTable(C.Structure):
     _fields_ = [("shard_weight", C.c_void_p * 8), ("num_shards", C.c_int32), ("rows_per_shard", C.c_int64),
                 ("rows", C.c_int64), ("ld", C.c_int64), ("indices", C.c_void_p), ("offsets", C.c_void_p),
-                ("nnz", C.c_int64), ("out_off", C.c_int64), ("out_stride", C.c_int64)]
+                ("nnz", C.c_int64), ("out_off", C.c_int64), ("out_stride", C.c_int64), ("weight_dtype", C.c_int32)]
 
 
 class EmbDedup(C.Structure):

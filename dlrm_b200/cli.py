@@ -91,6 +91,8 @@ def build_parser():
                    default="random")
     # dlrm_b200 addition (not in the reference): GEMM back end
     p.add_argument("--gemm", type=str, default="tc", choices=["tc", "tc_bf16", "simt"])
+    # dlrm_b200 addition: storage type of the embedding tables (fp16: stochastically rounded row updates)
+    p.add_argument("--emb-dtype", type=str, default="fp32", choices=["fp32", "fp16"])
     return p
 
 
@@ -224,7 +226,8 @@ def run(argv=None):
                     sigmoid_top=ln_top.size - 2, sync_dense_params=args.sync_dense_params,
                     loss_threshold=args.loss_threshold, ndevices=-1, weighted_pooling=args.weighted_pooling,
                     loss_function=args.loss_function, device=device, gemm=args.gemm,
-                    max_batch=args.mini_batch_size, loss_weights=loss_ws)
+                    max_batch=args.mini_batch_size, loss_weights=loss_ws,
+                    emb_dtype=torch.float16 if args.emb_dtype == "fp16" else torch.float32)
     optimizer = lr_scheduler = None
     if not args.inference_only:
         if args.optimizer == "sgd":

@@ -1,5 +1,6 @@
 // Shared helpers for libdlrm_b200.so (sm_90a only).
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -78,6 +79,81 @@ __device__ __forceinline__ float4 ldg_stream_f4(const float* p) {
                : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
                : "l"(p));
   return v;
+}
+
+// ---- fp16 table rows (weight_dtype = DLRM_DTYPE_F16): widened to fp32 on load, stochastically rounded on store.
+// The kernels are templated on the row type `wt` (float or __half); the float instantiations are the fp32 code.
+template <typename wt>
+struct is_f16 { static constexpr bool value = false; };
+template <>
+struct is_f16<__half> { static constexpr bool value = true; };
+
+__device__ __forceinline__ float4 h4_to_f4(uint2 u) {
+  const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u.x));
+  const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
+  return make_float4(a.x, a.y, b.x, b.y);
+}
+
+// 4 consecutive row elements as fp32 (16-byte fp32 / 8-byte fp16 load)
+template <typename wt>
+__device__ __forceinline__ float4 ld_row4(const wt* p) {
+  if constexpr (is_f16<wt>::value) return h4_to_f4(*reinterpret_cast<const uint2*>(p));
+  else return *reinterpret_cast<const float4*>(p);
+}
+// the same through the non-allocating read-only path (gather)
+template <typename wt>
+__device__ __forceinline__ float4 ldg_stream_row4(const wt* p) {
+  if constexpr (is_f16<wt>::value) {
+    uint2 u;
+    asm("ld.global.nc.L1::no_allocate.v2.u32 {%0,%1}, [%2];" : "=r"(u.x), "=r"(u.y) : "l"(p));
+    return h4_to_f4(u);
+  } else {
+    return ldg_stream_f4(p);
+  }
+}
+
+// finaliser of splitmix64 (dlrm_b200/mlperf.py; the synthetic batches of shard_ops.cu use it too)
+__device__ __forceinline__ unsigned long long splitmix64(unsigned long long x) {
+  x += 0x9E3779B97F4A7C15ull;
+  x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
+  x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
+  return x ^ (x >> 31);
+}
+// key of a global row for the stochastic rounding of its columns (include/dlrm_b200.h, round_key)
+__device__ __forceinline__ unsigned long long sr_row_key(unsigned long long round_key, long long global_row) {
+  return round_key ^ ((unsigned long long)global_row * 0xC2B2AE3D27D4EB4Full);
+}
+// 64 random bits for columns [4 q, 4 q + 4) of a row: column 4 q + j uses bits [16 j, 16 j + 16)
+__device__ __forceinline__ unsigned long long sr_bits(unsigned long long row_key, int q) {
+  return splitmix64(row_key ^ ((unsigned long long)q * 0x165667B19E3779F9ull));
+}
+
+// Stochastic rounding of fp32 x to fp16 with the 16 random bits r (the definition in include/dlrm_b200.h).
+__device__ __forceinline__ unsigned short f32_to_f16_sr(float x, unsigned r) {
+  const float ax = fabsf(x);
+  const unsigned short sign = (__float_as_uint(x) >> 16) & 0x8000u;
+  if (!(ax <= 65504.f)) return (ax != ax) ? (unsigned short)(sign | 0x7e00u) : (unsigned short)(sign | 0x7c00u);
+  const unsigned short lo = __half_as_ushort(__float2half_rz(x));   // the fp16 neighbour toward zero
+  const float flo = fabsf(__half2float(__ushort_as_half(lo)));
+  if (flo == ax) return lo;
+  const float fhi = fabsf(__half2float(__ushort_as_half((unsigned short)(lo + 1))));   // away from zero
+  const float t = floorf((ax - flo) / (fhi - flo) * 65536.f);       // exact: the step is a power of two
+  return ((float)r < t) ? (unsigned short)(lo + 1) : lo;
+}
+
+// store 4 consecutive fp32 values as row elements: fp32 as is, fp16 with stochastic rounding from `bits`
+template <typename wt>
+__device__ __forceinline__ void st_row4(wt* p, float4 v, unsigned long long bits) {
+  if constexpr (is_f16<wt>::value) {
+    const unsigned a = f32_to_f16_sr(v.x, (unsigned)(bits & 0xffffu));
+    const unsigned b = f32_to_f16_sr(v.y, (unsigned)((bits >> 16) & 0xffffu));
+    const unsigned c = f32_to_f16_sr(v.z, (unsigned)((bits >> 32) & 0xffffu));
+    const unsigned d = f32_to_f16_sr(v.w, (unsigned)(bits >> 48));
+    *reinterpret_cast<uint2*>(p) = make_uint2(a | (b << 16), c | (d << 16));
+  } else {
+    (void)bits;
+    *reinterpret_cast<float4*>(p) = v;
+  }
 }
 
 // slot of a (table,row) in the duplicate filter: the address of the row's list head is a unique key

@@ -27,6 +27,9 @@
 //            head[row] = 0 together.  Two random DRAM accesses per updated row: row + words in,
 //            row + words out.  Non-owners do nothing.  Rows without duplicates (the common case at
 //            1e6-row tables) never touch link[] beyond their own entry.
+//   fp16 tables (template row type wt = __half): the owner widens the row to fp32, applies the same fp32 step and
+//            stores the row with stochastic rounding (st_row4, common.cuh); the accumulator and the head stay
+//            fp32 / int32 words behind the row.  The float instantiations are the fp32 kernels.
 #include "common.cuh"
 
 namespace dlrm {
@@ -147,14 +150,14 @@ __device__ __forceinline__ void list_sum_exact(const int2* link, int nxt, int se
 }
 
 struct EmbBwdTable {
-  float* w;
+  void* w;               // rows of the row type (float or __half)
   float* mom;
   int* head;
   const void* idx;
   const void* off;
   long long nnz;
   long long pair_base;
-  long long ld;          // row stride of w in floats
+  long long ld;          // row stride of w in elements of the row type
   long long mom_stride;  // elements between consecutive rows' accumulators
   long long hs;          // elements between consecutive rows' list heads
   long long dy_off;      // the dY row of (bag, this table) is dy_row(bag) + dy_off
@@ -184,6 +187,9 @@ struct EmbBwdParams {
   const unsigned char* flags;
   int debug;   // TIMING EXPERIMENTS ONLY (tunable upd_debug): 1 = no weight store, 2 = no weight load, 4 = no
                // accumulator / list-head stores, 8 = no gradient load.  Results are wrong when non-zero.
+  // fp16 tables: stochastic-rounding key of table k for this step (kept out of EmbBwdTable, so that the fp32
+  // kernels see the parameter layout they always had)
+  unsigned long long round_key[DLRM_B200_MAX_TABLES_PER_CALL];
 };
 
 __device__ __forceinline__ const float* dy_row(const EmbBwdParams& P, long long bag) {
@@ -238,10 +244,14 @@ struct Pack {
   float x[W];
 };
 
-template <int W>
-__device__ __forceinline__ Pack<W> ld_pack(const float* p) {
+template <int W, typename wt = float>
+__device__ __forceinline__ Pack<W> ld_pack(const wt* p) {
   Pack<W> r;
-  if (W == 4) {
+  if constexpr (is_f16<wt>::value) {
+    static_assert(W == 4, "fp16 rows take the 4-wide path");
+    const float4 v = ld_row4(p);
+    r.x[0] = v.x; r.x[1 % W] = v.y; r.x[2 % W] = v.z; r.x[3 % W] = v.w;
+  } else if (W == 4) {
     const float4 v = *reinterpret_cast<const float4*>(p);
     r.x[0] = v.x; r.x[1 % W] = v.y; r.x[2 % W] = v.z; r.x[3 % W] = v.w;
   } else {
@@ -249,9 +259,11 @@ __device__ __forceinline__ Pack<W> ld_pack(const float* p) {
   }
   return r;
 }
-template <int W>
-__device__ __forceinline__ void st_pack(float* p, const Pack<W>& r) {
-  if (W == 4) {
+template <int W, typename wt = float>
+__device__ __forceinline__ void st_pack(wt* p, const Pack<W>& r, unsigned long long bits = 0) {
+  if constexpr (is_f16<wt>::value) {
+    st_row4(p, make_float4(r.x[0], r.x[1 % W], r.x[2 % W], r.x[3 % W]), bits);
+  } else if (W == 4) {
     *reinterpret_cast<float4*>(p) = make_float4(r.x[0], r.x[1 % W], r.x[2 % W], r.x[3 % W]);
   } else {
     *p = r.x[0];
@@ -367,7 +379,7 @@ __device__ __noinline__ void dup_sum_long(const EmbBwdParams& P, int nxt, int se
     for (int e = 0; e < W; ++e) g[v].x[e] = acc[v * W + e];
 }
 
-template <int W, int NV, typename idx_t>
+template <typename wt, int W, int NV, typename idx_t>
 __global__ void __launch_bounds__(256, NV == 1 ? 3 : 1) emb_update_kernel(const __grid_constant__ EmbBwdParams P,
                                                                           int num_tables, long long total_hint) {
   __shared__ long long bound[DLRM_B200_MAX_TABLES_PER_CALL + 1], tend[DLRM_B200_MAX_TABLES_PER_CALL + 1];
@@ -419,7 +431,7 @@ __global__ void __launch_bounds__(256, NV == 1 ? 3 : 1) emb_update_kernel(const 
         const int bag = __shfl_sync(0xffffffffu, my_link.y, src);
         if ((owners >> src) & 1u) {
           const EmbBwdTable& tb = P.t[ku];
-          const float* wrow = tb.w + r * tb.ld;
+          const wt* wrow = static_cast<const wt*>(tb.w) + r * tb.ld;
           const float* grow = dy_row(P, bag) + tb.dy_off;
 #pragma unroll
           for (int v = 0; v < NV; ++v)
@@ -439,8 +451,10 @@ __global__ void __launch_bounds__(256, NV == 1 ? 3 : 1) emb_update_kernel(const 
         const int self_bag = __shfl_sync(0xffffffffu, my_link.y, src);
         if (!((owners >> src) & 1u)) continue;
         const EmbBwdTable& tb = P.t[ku];
-        float* wrow = tb.w + r * tb.ld;
+        wt* wrow = static_cast<wt*>(tb.w) + r * tb.ld;
         const long long dyk_off = tb.dy_off;
+        // fp16: random bits of column group q = lane + 32 v (columns 4q..4q+3) of this global row
+        const unsigned long long rkey = is_f16<wt>::value ? sr_row_key(P.round_key[ku], r + tb.row_lo) : 0ull;
         Pack<W> w[NV], g[NV];
 #pragma unroll
         for (int v = 0; v < NV; ++v) { w[v] = wpf[u][v]; g[v] = gpf[u][v]; }
@@ -497,7 +511,7 @@ __global__ void __launch_bounds__(256, NV == 1 ? 3 : 1) emb_update_kernel(const 
             if (col_ok[v]) {
 #pragma unroll
               for (int e = 0; e < W; ++e) w[v].x[e] = fmaf(nlr, g[v].x[e] / stdv, w[v].x[e]);
-              st_pack<W>(wrow + lane * W + v * 32 * W, w[v]);
+              st_pack<W>(wrow + lane * W + v * 32 * W, w[v], is_f16<wt>::value ? sr_bits(rkey, lane + 32 * v) : 0ull);
             }
           if (lane == 0) tb.mom[r * tb.mom_stride] = m_new;
         } else {
@@ -507,7 +521,7 @@ __global__ void __launch_bounds__(256, NV == 1 ? 3 : 1) emb_update_kernel(const 
             if (col_ok[v]) {
 #pragma unroll
               for (int e = 0; e < W; ++e) w[v].x[e] = fmaf(nlr, g[v].x[e], w[v].x[e]);
-              st_pack<W>(wrow + lane * W + v * 32 * W, w[v]);
+              st_pack<W>(wrow + lane * W + v * 32 * W, w[v], is_f16<wt>::value ? sr_bits(rkey, lane + 32 * v) : 0ull);
             }
         }
         if (lane == 0 && ((susp_mask >> src) & 1u)) tb.head[r * tb.hs] = 0;
@@ -535,7 +549,7 @@ __global__ void __launch_bounds__(256, NV == 1 ? 3 : 1) emb_update_kernel(const 
 //   * rows with duplicates (rare at large tables) take an out-of-line path.
 // ---------------------------------------------------------------------------------------------
 struct UpdTableS {
-  float* w;
+  void* w;
   float* mom;
   int* head;
   unsigned char* mark;
@@ -593,7 +607,7 @@ __device__ __noinline__ float4 upd_sum_duplicates(const EmbBwdParams& P, int nxt
   return g;
 }
 
-template <typename idx_t, int PF, int MINB>      // PF: row PAIRS in flight per warp
+template <typename wt, typename idx_t, int PF, int MINB>      // PF: row PAIRS in flight per warp
 __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid_constant__ EmbBwdParams P, int num_tables,
                                                                     long long total_hint) {
   __shared__ long long bound[DLRM_B200_MAX_TABLES_PER_CALL + 1], tend[DLRM_B200_MAX_TABLES_PER_CALL + 1];
@@ -609,7 +623,7 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
   const int D = P.dim;
   const int lane = threadIdx.x & 31;
   // Rows WITHOUT duplicates (almost all of them at large tables) are processed TWO per warp step: lanes 0-15
-  // take one row, lanes 16-31 another, 8 columns (two float4) per lane.  Every shuffle / FMA / branch of the
+  // take one row, lanes 16-31 another, 8 columns (two float4; one 16-byte load of an fp16 row) per lane.  Every shuffle / FMA / branch of the
   // step then serves two rows, and twice as many rows are in flight per warp.
   const int half = lane >> 4, l16 = lane & 15;
   const bool c0_ok = l16 * 8 < D, c1_ok = l16 * 8 + 4 < D;
@@ -642,7 +656,10 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
       r = (int)rr;
     }
     const int nxt = owner ? lk.x : 0, bag = lk.y;
-    float* wptr = owner ? tb.w + (long long)r * tb.ld : nullptr;
+    wt* wptr = owner ? static_cast<wt*>(tb.w) + (long long)r * tb.ld : nullptr;
+    // fp16: the key of the owned GLOBAL row for the stochastic rounding of its columns
+    const unsigned long long rkey =
+        (is_f16<wt>::value && owner) ? sr_row_key(P.round_key[k], (long long)r + tb.row_lo) : 0ull;
     const float* gptr = owner ? dy_row(P, bag) + tb.dy_off : nullptr;
     float* mptr = (owner && adagrad) ? tb.mom + (long long)r * tb.mom_stride : nullptr;
     int* hptr = owner ? tb.head + (long long)r * tb.hs : nullptr;
@@ -662,12 +679,22 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
         simple &= simple - 1u;
         const int s_ = half ? sb[u] : sa[u];
         const int sc = s_ < 0 ? 0 : s_;
-        const float* wp = reinterpret_cast<const float*>(__shfl_sync(0xffffffffu, (unsigned long long)wptr, sc)) + l16 * 8;
+        const wt* wp = reinterpret_cast<const wt*>(__shfl_sync(0xffffffffu, (unsigned long long)wptr, sc)) + l16 * 8;
         const float* gp = reinterpret_cast<const float*>(__shfl_sync(0xffffffffu, (unsigned long long)gptr, sc)) + l16 * 8;
         const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
         const bool ldw = !(dbg & 2), ldg = !(dbg & 8);
-        wv[u][0] = (s_ >= 0 && c0_ok && ldw) ? *reinterpret_cast<const float4*>(wp) : z;
-        wv[u][1] = (s_ >= 0 && c1_ok && ldw) ? *reinterpret_cast<const float4*>(wp + 4) : z;
+        if constexpr (is_f16<wt>::value) {      // 8 halves = one 16-byte load (c1_ok == c0_ok: dim % 8 == 0)
+          if (s_ >= 0 && c0_ok && ldw) {
+            const uint4 h = *reinterpret_cast<const uint4*>(wp);
+            wv[u][0] = h4_to_f4(make_uint2(h.x, h.y));
+            wv[u][1] = h4_to_f4(make_uint2(h.z, h.w));
+          } else {
+            wv[u][0] = z; wv[u][1] = z;
+          }
+        } else {
+          wv[u][0] = (s_ >= 0 && c0_ok && ldw) ? *reinterpret_cast<const float4*>(wp) : z;
+          wv[u][1] = (s_ >= 0 && c1_ok && ldw) ? *reinterpret_cast<const float4*>(wp + 4) : z;
+        }
         gv[u][0] = (s_ >= 0 && c0_ok && ldg) ? *reinterpret_cast<const float4*>(gp) : z;
         gv[u][1] = (s_ >= 0 && c1_ok && ldg) ? *reinterpret_cast<const float4*>(gp + 4) : z;
         // the owning lanes load their accumulators in the same batch as the rows
@@ -691,8 +718,21 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
           if (lane == sa[u] && !(dbg & 4)) *mptr = mA;               // the owning lanes store their accumulators
           if (lane == sb[u] && !(dbg & 4)) *mptr = mB;
         }
-        float* wp = reinterpret_cast<float*>(__shfl_sync(0xffffffffu, (unsigned long long)wptr, sc)) + l16 * 8;
-        if (s_ >= 0) {
+        wt* wp = reinterpret_cast<wt*>(__shfl_sync(0xffffffffu, (unsigned long long)wptr, sc)) + l16 * 8;
+        if constexpr (is_f16<wt>::value) {
+          const unsigned long long rk = __shfl_sync(0xffffffffu, rkey, sc);
+          if (s_ >= 0) {
+            float4 w0 = wv[u][0], w1 = wv[u][1];
+            w0.x = fmaf(scale, g0.x, w0.x); w0.y = fmaf(scale, g0.y, w0.y); w0.z = fmaf(scale, g0.z, w0.z); w0.w = fmaf(scale, g0.w, w0.w);
+            w1.x = fmaf(scale, g1.x, w1.x); w1.y = fmaf(scale, g1.y, w1.y); w1.z = fmaf(scale, g1.z, w1.z); w1.w = fmaf(scale, g1.w, w1.w);
+            if (c0_ok && !(dbg & 1)) {
+              uint2 a, b;
+              st_row4(reinterpret_cast<__half*>(&a), w0, sr_bits(rk, l16 * 2));
+              st_row4(reinterpret_cast<__half*>(&b), w1, sr_bits(rk, l16 * 2 + 1));
+              *reinterpret_cast<uint4*>(wp) = make_uint4(a.x, a.y, b.x, b.y);
+            }
+          }
+        } else if (s_ >= 0) {
           float4 w0 = wv[u][0], w1 = wv[u][1];
           w0.x = fmaf(scale, g0.x, w0.x); w0.y = fmaf(scale, g0.y, w0.y); w0.z = fmaf(scale, g0.z, w0.z); w0.w = fmaf(scale, g0.w, w0.w);
           w1.x = fmaf(scale, g1.x, w1.x); w1.y = fmaf(scale, g1.y, w1.y); w1.z = fmaf(scale, g1.z, w1.z); w1.w = fmaf(scale, g1.w, w1.w);
@@ -710,8 +750,8 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
       const int nx = __shfl_sync(0xffffffffu, nxt, s_);
       const int sbg = __shfl_sync(0xffffffffu, bag, s_);
       const long long dyo = __shfl_sync(0xffffffffu, tb.dy_off, s_);       // the OWNER's table (windows may straddle)
-      float* wp = reinterpret_cast<float*>(__shfl_sync(0xffffffffu, (unsigned long long)wptr, s_));
-      float4 w = col_ok ? *reinterpret_cast<const float4*>(wp + lane * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
+      wt* wp = reinterpret_cast<wt*>(__shfl_sync(0xffffffffu, (unsigned long long)wptr, s_));
+      float4 w = col_ok ? ld_row4(wp + lane * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
       const float m_old = (adagrad && lane == s_) ? *mptr : 0.f;
       const float4 g = upd_sum_duplicates(P, nx, (int)(base + s_), sbg, dyo, lane, col_ok);
       float scale = nlr;
@@ -724,7 +764,12 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
       }
       w.x = fmaf(scale, g.x, w.x); w.y = fmaf(scale, g.y, w.y);
       w.z = fmaf(scale, g.z, w.z); w.w = fmaf(scale, g.w, w.w);
-      if (col_ok) *reinterpret_cast<float4*>(wp + lane * 4) = w;
+      if constexpr (is_f16<wt>::value) {
+        const unsigned long long rk = __shfl_sync(0xffffffffu, rkey, s_);
+        if (col_ok) st_row4(wp + lane * 4, w, sr_bits(rk, lane));
+      } else {
+        if (col_ok) *reinterpret_cast<float4*>(wp + lane * 4) = w;
+      }
       if (lane == s_) *hptr = 0;
     }
   }
@@ -756,7 +801,12 @@ static int fill_params(EmbBwdParams& P, const dlrm_emb_bwd_table_t* tables, int 
     P.t[k].rows = tables[k].rows > 0 ? tables[k].rows : 0x7fffffffffffffffLL;
     P.t[k].row_lo = tables[k].row_n > 0 ? tables[k].row_lo : 0;
     P.t[k].row_n = tables[k].row_n > 0 ? tables[k].row_n : P.t[k].rows;
+    P.round_key[k] = tables[k].round_key;
+    if (tables[k].weight_dtype != tables[0].weight_dtype)
+      return set_error("%s: table %d: weight_dtype differs from table 0's (one row type per call)", who, k);
   }
+  if (num_tables > 0 && tables[0].weight_dtype != DLRM_DTYPE_F32 && tables[0].weight_dtype != DLRM_DTYPE_F16)
+    return set_error("%s: weight_dtype=%d", who, tables[0].weight_dtype);
   return 0;
 }
 
@@ -800,6 +850,9 @@ static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, i
   if (optimizer != DLRM_OPT_SGD && optimizer != DLRM_OPT_RWSADAGRAD)
     return set_error("emb_bwd_update: optimizer=%d", optimizer);
   if (dim <= 0 || dim > 1024) return set_error("emb_bwd_update: dim=%d unsupported (1..1024)", dim);
+  const bool f16 = num_tables > 0 && tables[0].weight_dtype == DLRM_DTYPE_F16;
+  if (f16 && dim % 8) return set_error("emb_bwd_update: fp16 tables need dim %% 8 == 0 (dim=%d)", dim);
+  bool lean_rows = true;
   if (num_tables == 0 || batch == 0) return 0;
   if (!next || (!dY && !peer_dY)) return set_error("emb_bwd_update: NULL next/dY");
   bool vec = (dim % 4 == 0) && (peer_dY || aligned16(dY)) && dy_stride_sample % 4 == 0 && dy_stride_table % 4 == 0;
@@ -828,6 +881,9 @@ static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, i
     if (P.t[k].ld <= 0) P.t[k].ld = dim;
     if (P.t[k].ld < dim) return set_error("emb_bwd_update: table %d: ld < dim", k);
     vec = vec && (P.t[k].ld % 4 == 0);
+    // the lean kernel moves 8 columns per lane in one 16-byte access: fp16 rows must start on 16-byte boundaries
+    // (ld % 8 halves); fp16 rows that are only 8-byte aligned take the general kernel (8-byte accesses)
+    lean_rows = lean_rows && (!f16 || P.t[k].ld % 8 == 0);
   }
   P.link = reinterpret_cast<int2*>(const_cast<int32_t*>(next));
   P.dY = dY;
@@ -856,26 +912,42 @@ static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, i
   if (gridx < 1) gridx = 1;
   const long long total_hint = include_last ? 0 : (tables[num_tables - 1].pair_base + tables[num_tables - 1].nnz);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-#define UPD(Wd, NV)                                                                                        \
+#define UPD_T(WT, Wd, NV)                                                                                  \
   do {                                                                                                     \
     if (idx_bytes == 8)                                                                                    \
-      emb_update_kernel<Wd, NV, long long><<<(unsigned)gridx, block, 0, st>>>(P, num_tables, total_hint);  \
+      emb_update_kernel<WT, Wd, NV, long long><<<(unsigned)gridx, block, 0, st>>>(P, num_tables, total_hint); \
     else                                                                                                   \
-      emb_update_kernel<Wd, NV, int><<<(unsigned)gridx, block, 0, st>>>(P, num_tables, total_hint);        \
+      emb_update_kernel<WT, Wd, NV, int><<<(unsigned)gridx, block, 0, st>>>(P, num_tables, total_hint);    \
     DLRM_CHECK_LAUNCH("emb_update_kernel");                                                                \
     return 0;                                                                                              \
   } while (0)
-  if (vec && dim <= 128 && !P.flags && get_tunable(TUNE_UPD_LEAN) != 2) {
+#define UPD(Wd, NV) UPD_T(float, Wd, NV)
+  if (f16 && !vec)
+    return set_error("emb_bwd_update: fp16 tables need a 16-byte aligned weight pointer, ld %% 4 == 0 (8-byte rows) "
+                     "and 16-byte aligned gradient rows");
+  if (vec && lean_rows && dim <= 128 && !P.flags && get_tunable(TUNE_UPD_LEAN) != 2) {
     long long gl = (total / 32 + block / 32) / (block / 32);
     if (gl > (long long)sms * 3) gl = (long long)sms * 3;
     if (gl < 1) gl = 1;
     // 3 CTAs of 256 threads per SM (<= 85 registers), 2 row pairs in flight per warp: on H100 (cfg3) 3 pairs /
     // 3 CTAs and 4 pairs / 2 CTAs per SM were measured no faster and 8 % slower.  The kernel is bound by the RATE of random accesses
     // (row + accumulator read, row + accumulator + head write), not by the latency of any one of them.
-    if (idx_bytes == 8) emb_update_lean_kernel<long long, 2, 3><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);
-    else emb_update_lean_kernel<int, 2, 3><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);
+    if (f16) {
+      if (idx_bytes == 8) emb_update_lean_kernel<__half, long long, 2, 3><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);
+      else emb_update_lean_kernel<__half, int, 2, 3><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);
+    } else if (idx_bytes == 8) {
+      emb_update_lean_kernel<float, long long, 2, 3><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);
+    } else {
+      emb_update_lean_kernel<float, int, 2, 3><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);
+    }
     DLRM_CHECK_LAUNCH("emb_update_lean_kernel");
     return 0;
+  }
+  if (f16) {
+    if (dim <= 128) UPD_T(__half, 4, 1);
+    if (dim <= 256) UPD_T(__half, 4, 2);
+    if (dim <= 512) UPD_T(__half, 4, 4);
+    UPD_T(__half, 4, 8);
   }
   if (vec) {
     if (dim <= 128) UPD(4, 1);
@@ -890,6 +962,7 @@ static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, i
   if (dim <= 512) UPD(1, 16);
   UPD(1, 32);
 #undef UPD
+#undef UPD_T
 }
 
 extern "C" int dlrm_b200_emb_bwd_update(const dlrm_emb_bwd_table_t* tables, int num_tables, int dim,

@@ -9,12 +9,14 @@
 // with one coalesced load per G positions and broadcast with warp shuffles), (b) the indices
 // of the next bag being prefetched while the rows of the current bag are in flight, and
 // (c) 8..16 warps per CTA x many CTAs per SM.
+// fp16 tables (template row type wt = __half): the same lanes load 4 halves (8 bytes) instead of a float4 and
+// widen them, so every column is still summed in fp32 in index order (== the fp32 gather over the widened table).
 #include "common.cuh"
 
 namespace dlrm {
 
 struct EmbFwdTable {
-  const float* w;
+  const void* w;        // rows of the table's row type (float or __half)
   const void* idx;
   const void* off;
   const float* rw;
@@ -24,7 +26,7 @@ struct EmbFwdTable {
                         // head lives inside the row's own DRAM page: [weights | accumulator | head | pad])
   long long pair_base;  // training: first slot of this table in link[]
   unsigned char* mark;  // training: superseded marks, indexed like link[] (see emb_bwd.cu)
-  long long ld;         // row stride in floats
+  long long ld;         // row stride in elements of the row type
   long long out_off;    // pooled row of bag b goes to out_row(b) [+ b_local * out_stride] + out_off
   long long out_stride; // elements between consecutive samples of THIS table's output
   long long rows;       // rows of the whole table: an index outside [0, rows) is an error
@@ -88,7 +90,7 @@ __device__ __forceinline__ long long bag_end(const idx_t* off, long long b, long
 // G lanes per bag, NV float4 per lane (dim = 4*G*NV when exact; columns >= dim are masked).
 // grid = (groups of S bags, table): a plain grid at 64 registers / 4 CTAs per SM rather than a persistent one-wave
 // grid with more registers per thread -- the gather is latency-bound, so resident warps matter most.
-template <int G, int NV, int U, typename idx_t, bool WEIGHTED, bool LINK>
+template <typename wt, int G, int NV, int U, typename idx_t, bool WEIGHTED, bool LINK>
 __global__ void __launch_bounds__(256, (G == 32 && NV == 1) ? 4 : 1) emb_fwd_vec_kernel(
     const __grid_constant__ EmbFwdParams P, int num_tables) {
   const int D = P.dim;
@@ -103,7 +105,7 @@ __global__ void __launch_bounds__(256, (G == 32 && NV == 1) ? 4 : 1) emb_fwd_vec
     const EmbFwdTable& tb = P.t[table];
     const idx_t* __restrict__ idx = static_cast<const idx_t*>(tb.idx);
     const idx_t* __restrict__ off = static_cast<const idx_t*>(tb.off);
-    const float* __restrict__ W = tb.w;
+    const wt* __restrict__ W = static_cast<const wt*>(tb.w);
     const long long b0 =
         (((long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * GROUPS_PER_WARP + grp) * S;
     if (b0 >= P.batch) return;
@@ -160,10 +162,10 @@ __global__ void __launch_bounds__(256, (G == 32 && NV == 1) ? 4 : 1) emb_fwd_vec
           for (int u = 0; u < U; ++u) {
             const long long r = __shfl_sync(gmask, my_row, jj + u, G);  // jj+u < G always (U | G)
             if (jj + u < n) {
-              const float* rp = W + r * tb.ld + gl * 4;
+              const wt* rp = W + r * tb.ld + gl * 4;
 #pragma unroll
               for (int v = 0; v < NV; ++v) {
-                if (gl * 4 + v * G * 4 < D) val[u][v] = ldg_stream_f4(rp + v * G * 4);
+                if (gl * 4 + v * G * 4 < D) val[u][v] = ldg_stream_row4(rp + v * G * 4);
               }
               if (WEIGHTED) wgt[u] = __ldg(tb.rw + r);
             }
@@ -210,7 +212,7 @@ __global__ void __launch_bounds__(256, (G == 32 && NV == 1) ? 4 : 1) emb_fwd_vec
 // global batch, only the indices that fall into its range (a partial sum; the N partials of a bag are added on the
 // rank that owns the sample).  The indices of a 32-wide chunk that are "mine" are compacted with a ballot so
 // that up to U row loads stay in flight however sparse the hits are (L = 100 over 8 shards: ~4 of 32).
-template <int G, int NV, int U, typename idx_t, bool WEIGHTED, bool LINK>
+template <typename wt, int G, int NV, int U, typename idx_t, bool WEIGHTED, bool LINK>
 __global__ void __launch_bounds__(256) emb_fwd_shard_kernel(const __grid_constant__ EmbFwdParams P, int num_tables) {
   const int D = P.dim;
   constexpr int GROUPS_PER_WARP = 32 / G;
@@ -222,7 +224,7 @@ __global__ void __launch_bounds__(256) emb_fwd_shard_kernel(const __grid_constan
   const EmbFwdTable& tb = P.t[blockIdx.y];
   const idx_t* __restrict__ idx = static_cast<const idx_t*>(tb.idx);
   const idx_t* __restrict__ off = static_cast<const idx_t*>(tb.off);
-  const float* __restrict__ W = tb.w;
+  const wt* __restrict__ W = static_cast<const wt*>(tb.w);
   const bool link_tb = LINK && tb.head != nullptr;
   const int S = P.bags_per_group;
   const long long b0 = (((long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * GROUPS_PER_WARP + grp) * S;
@@ -257,10 +259,10 @@ __global__ void __launch_bounds__(256) emb_fwd_shard_kernel(const __grid_constan
           live &= live - 1u;                      // clears the lowest set bit (0 stays 0)
           const long long r = __shfl_sync(gmask, lr, src, G);
           if (on[u]) {
-            const float* rp = W + r * tb.ld + gl * 4;
+            const wt* rp = W + r * tb.ld + gl * 4;
 #pragma unroll
             for (int v = 0; v < NV; ++v)
-              if (gl * 4 + v * G * 4 < D) val[u][v] = ldg_stream_f4(rp + v * G * 4);
+              if (gl * 4 + v * G * 4 < D) val[u][v] = ldg_stream_row4(rp + v * G * 4);
             if (WEIGHTED) wgt[u] = __ldg(tb.rw + r);
           }
         }
@@ -298,7 +300,7 @@ __global__ void __launch_bounds__(256) emb_fwd_shard_kernel(const __grid_constan
 // 512-byte NVLink reads, up to U in flight per lane group.  No partial sums, no reduction; NVLink carries
 // L x 512 B per sample instead of (N-1) x 512 B of partial sums (better for short bags, worse for L = 100).
 struct EmbRemoteTable {
-  const float* shard_w[DLRM_B200_MAX_PEERS];   // base of shard s (rows [s*rps, (s+1)*rps))
+  const void* shard_w[DLRM_B200_MAX_PEERS];   // base of shard s (rows [s*rps, (s+1)*rps))
   const void* idx;
   const void* off;
   long long nnz, ld, out_off, out_stride, rows, rps;
@@ -311,7 +313,7 @@ struct EmbRemoteParams {
   unsigned* err;
 };
 
-template <int G, int NV, int U, typename idx_t>
+template <typename wt, int G, int NV, int U, typename idx_t>
 __global__ void __launch_bounds__(256) emb_fwd_remote_kernel(const __grid_constant__ EmbRemoteParams P) {
   const int D = P.dim;
   constexpr int GROUPS_PER_WARP = 32 / G;
@@ -346,10 +348,10 @@ __global__ void __launch_bounds__(256) emb_fwd_remote_kernel(const __grid_consta
           const long long r = __shfl_sync(gmask, my_row, jj + u, G);
           if (jj + u < n) {
             const long long sh = r / tb.rps;
-            const float* rp = tb.shard_w[sh] + (r - sh * tb.rps) * tb.ld + gl * 4;
+            const wt* rp = static_cast<const wt*>(tb.shard_w[sh]) + (r - sh * tb.rps) * tb.ld + gl * 4;
 #pragma unroll
             for (int v = 0; v < NV; ++v)
-              if (gl * 4 + v * G * 4 < D) val[u][v] = ldg_stream_f4(rp + v * G * 4);
+              if (gl * 4 + v * G * 4 < D) val[u][v] = ldg_stream_row4(rp + v * G * 4);
           }
         }
 #pragma unroll
@@ -371,7 +373,7 @@ __global__ void __launch_bounds__(256) emb_fwd_remote_kernel(const __grid_consta
 }
 
 // any dim / any alignment: one thread per output element, sequential over the bag
-template <typename idx_t, bool WEIGHTED, bool LINK>
+template <typename wt, typename idx_t, bool WEIGHTED, bool LINK>
 __global__ void emb_fwd_scalar_kernel(const __grid_constant__ EmbFwdParams P) {
   const EmbFwdTable& tb = P.t[blockIdx.y];
   const idx_t* __restrict__ idx = static_cast<const idx_t*>(tb.idx);
@@ -395,29 +397,29 @@ __global__ void emb_fwd_scalar_kernel(const __grid_constant__ EmbFwdParams P) {
       if (prev) tb.mark[prev - 1] = 1;
     }
     if (!mine) continue;
-    const float x = tb.w[r * tb.ld + d];
+    const float x = (float)static_cast<const wt*>(tb.w)[r * tb.ld + d];
     acc = WEIGHTED ? fmaf(tb.rw[r], x, acc) : acc + x;
   }
   out_ptr(P, tb, b)[d] = acc;
 }
 
-template <int G, int NV, int U, typename idx_t, bool WEIGHTED, bool LINK>
+template <typename wt, int G, int NV, int U, typename idx_t, bool WEIGHTED, bool LINK>
 static int launch_vec(const EmbFwdParams& P, int num_tables, bool shard, cudaStream_t st) {
   const int block = 256;
   const long long groups_per_block = (long long)(block / 32) * (32 / G);
   const long long groups = (P.batch + P.bags_per_group - 1) / P.bags_per_group;
   dim3 grid((unsigned)((groups + groups_per_block - 1) / groups_per_block), (unsigned)num_tables);
   if (shard) {
-    emb_fwd_shard_kernel<G, NV, U, idx_t, WEIGHTED, LINK><<<grid, block, 0, st>>>(P, num_tables);
+    emb_fwd_shard_kernel<wt, G, NV, U, idx_t, WEIGHTED, LINK><<<grid, block, 0, st>>>(P, num_tables);
     DLRM_CHECK_LAUNCH("emb_fwd_shard_kernel");
     return 0;
   }
-  emb_fwd_vec_kernel<G, NV, U, idx_t, WEIGHTED, LINK><<<grid, block, 0, st>>>(P, num_tables);
+  emb_fwd_vec_kernel<wt, G, NV, U, idx_t, WEIGHTED, LINK><<<grid, block, 0, st>>>(P, num_tables);
   DLRM_CHECK_LAUNCH("emb_fwd_vec_kernel");
   return 0;
 }
 
-template <typename idx_t, bool WEIGHTED, bool LINK>
+template <typename wt, typename idx_t, bool WEIGHTED, bool LINK>
 static int dispatch(const EmbFwdParams& Pin, int num_tables, bool vec_ok, bool shard, cudaStream_t st) {
   EmbFwdParams P = Pin;
   const int D = P.dim;
@@ -428,8 +430,8 @@ static int dispatch(const EmbFwdParams& Pin, int num_tables, bool vec_ok, bool s
 #define VEC(G, NV)                                                                   \
   do {                                                                               \
     P.bags_per_group = S < (G) ? S : (G)-1;                                          \
-    if ((G) >= 8 && u8) return launch_vec<G, NV, 8, idx_t, WEIGHTED, LINK>(P, num_tables, shard, st); \
-    return launch_vec<G, NV, ((G) >= 4 ? 4 : (G)), idx_t, WEIGHTED, LINK>(P, num_tables, shard, st);  \
+    if ((G) >= 8 && u8) return launch_vec<wt, G, NV, 8, idx_t, WEIGHTED, LINK>(P, num_tables, shard, st); \
+    return launch_vec<wt, G, NV, ((G) >= 4 ? 4 : (G)), idx_t, WEIGHTED, LINK>(P, num_tables, shard, st);  \
   } while (0)
     if (D == 16) VEC(4, 1);  // dim 4 / 8: scalar kernel (a group must hold S+1 bag bounds)
     if (D == 32) VEC(8, 1);
@@ -442,7 +444,7 @@ static int dispatch(const EmbFwdParams& Pin, int num_tables, bool vec_ok, bool s
   const int block = 256;
   const long long n = P.batch * D;
   dim3 grid((unsigned)((n + block - 1) / block), (unsigned)num_tables);
-  emb_fwd_scalar_kernel<idx_t, WEIGHTED, LINK><<<grid, block, 0, st>>>(P);
+  emb_fwd_scalar_kernel<wt, idx_t, WEIGHTED, LINK><<<grid, block, 0, st>>>(P);
   DLRM_CHECK_LAUNCH("emb_fwd_scalar_kernel");
   return 0;
 }
@@ -466,9 +468,14 @@ static int emb_fwd_impl(const dlrm_emb_fwd_table_t* tables, const dlrm_emb_bwd_t
   if (train && !link) return set_error("emb_bag_fwd_train: link is NULL");
   EmbFwdParams P;
   bool weighted = false, any_unweighted = false, any_shard = false;
+  const int dtype = num_tables > 0 ? tables[0].weight_dtype : DLRM_DTYPE_F32;
+  if (dtype != DLRM_DTYPE_F32 && dtype != DLRM_DTYPE_F16) return set_error("emb_bag_fwd: weight_dtype=%d", dtype);
+  if (dtype == DLRM_DTYPE_F16 && dim % 8) return set_error("emb_bag_fwd: fp16 tables need dim %% 8 == 0 (dim=%d)", dim);
   bool vec_ok = (dim % 4 == 0) && dim <= 512 && (peer_out || aligned16(out)) && out_stride_sample % 4 == 0 &&
                 out_stride_table % 4 == 0;
   for (int k = 0; k < num_tables; ++k) {
+    if (tables[k].weight_dtype != dtype)
+      return set_error("emb_bag_fwd: table %d: weight_dtype differs from table 0's (one row type per call)", k);
     P.t[k].w = tables[k].weight;
     P.t[k].idx = tables[k].indices;
     P.t[k].off = tables[k].offsets;
@@ -536,15 +543,19 @@ static int emb_fwd_impl(const dlrm_emb_fwd_table_t* tables, const dlrm_emb_bwd_t
     P.out = peer_out[0];
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-#define DISPATCH(IDX)                                                                          \
+#define DISPATCH(WT, IDX)                                                                      \
   do {                                                                                         \
-    if (train) return weighted ? dispatch<IDX, true, true>(P, num_tables, vec_ok, any_shard, st)          \
-                               : dispatch<IDX, false, true>(P, num_tables, vec_ok, any_shard, st);        \
-    return weighted ? dispatch<IDX, true, false>(P, num_tables, vec_ok, any_shard, st)                    \
-                    : dispatch<IDX, false, false>(P, num_tables, vec_ok, any_shard, st);                  \
+    if (train) return weighted ? dispatch<WT, IDX, true, true>(P, num_tables, vec_ok, any_shard, st)      \
+                               : dispatch<WT, IDX, false, true>(P, num_tables, vec_ok, any_shard, st);    \
+    return weighted ? dispatch<WT, IDX, true, false>(P, num_tables, vec_ok, any_shard, st)                \
+                    : dispatch<WT, IDX, false, false>(P, num_tables, vec_ok, any_shard, st);              \
   } while (0)
-  if (idx_bytes == 8) DISPATCH(long long);
-  DISPATCH(int);
+  if (dtype == DLRM_DTYPE_F16) {
+    if (idx_bytes == 8) DISPATCH(__half, long long);
+    DISPATCH(__half, int);
+  }
+  if (idx_bytes == 8) DISPATCH(float, long long);
+  DISPATCH(float, int);
 #undef DISPATCH
 }
 
@@ -588,8 +599,13 @@ extern "C" int dlrm_b200_emb_bag_fwd_remote(const dlrm_emb_remote_table_t* table
   if (!tables || !out) return set_error("emb_bag_fwd_remote: NULL pointer");
   if (dim <= 0 || dim % 4 || dim > 512 || !aligned16(out)) return set_error("emb_bag_fwd_remote: dim=%d (multiple of 4, <= 512)", dim);
   EmbRemoteParams P{};
+  const int dtype = tables[0].weight_dtype;
+  if (dtype != DLRM_DTYPE_F32 && dtype != DLRM_DTYPE_F16) return set_error("emb_bag_fwd_remote: weight_dtype=%d", dtype);
+  if (dtype == DLRM_DTYPE_F16 && dim % 8) return set_error("emb_bag_fwd_remote: fp16 tables need dim %% 8 == 0 (dim=%d)", dim);
   for (int k = 0; k < num_tables; ++k) {
     const dlrm_emb_remote_table_t& s = tables[k];
+    if (s.weight_dtype != dtype)
+      return set_error("emb_bag_fwd_remote: table %d: weight_dtype differs from table 0's (one row type per call)", k);
     if (s.num_shards < 1 || s.num_shards > DLRM_B200_MAX_PEERS || s.rows_per_shard <= 0 || s.rows <= 0 ||
         s.rows_per_shard * s.num_shards < s.rows)
       return set_error("emb_bag_fwd_remote: table %d: %d shards of %lld rows for %lld rows", k, s.num_shards,
@@ -609,11 +625,16 @@ extern "C" int dlrm_b200_emb_bag_fwd_remote(const dlrm_emb_remote_table_t* table
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 #define REMOTE(G, NV, IDX)                                                                                 \
   do {                                                                                                     \
+    if (dtype == DLRM_DTYPE_F16) REMOTE_T(__half, G, NV, IDX);                                             \
+    REMOTE_T(float, G, NV, IDX);                                                                           \
+  } while (0)
+#define REMOTE_T(WT, G, NV, IDX)                                                                           \
+  do {                                                                                                     \
     P.bags_per_group = 2;                                                                                  \
     const long long gpb = (256 / 32) * (32 / (G));                                                         \
     const long long groups = (batch + 1) / 2;                                                              \
     dim3 grid((unsigned)((groups + gpb - 1) / gpb), (unsigned)num_tables);                                 \
-    emb_fwd_remote_kernel<G, NV, ((G) >= 8 ? 8 : (G)), IDX><<<grid, 256, 0, st>>>(P);                       \
+    emb_fwd_remote_kernel<WT, G, NV, ((G) >= 8 ? 8 : (G)), IDX><<<grid, 256, 0, st>>>(P);                       \
     DLRM_CHECK_LAUNCH("emb_fwd_remote_kernel");                                                            \
     return 0;                                                                                              \
   } while (0)
@@ -630,4 +651,5 @@ extern "C" int dlrm_b200_emb_bag_fwd_remote(const dlrm_emb_remote_table_t* table
   REMOTE_D(int);
 #undef REMOTE_D
 #undef REMOTE
+#undef REMOTE_T
 }

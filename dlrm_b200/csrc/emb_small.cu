@@ -14,7 +14,8 @@
 //                to partial[chunk][row][:].
 //   apply      : one warp per row: sum the chunk partials in chunk order (= ascending position, the order
 //                grad.coalesce() sums duplicates in), then the same row update as emb_update_kernel.
-//                Rows nobody touched see g = 0 and are left bit-identical.
+//                Rows nobody touched see g = 0 and are left bit-identical.  fp16 tables (row type __half): the
+//                row is widened, updated in fp32 and stored with stochastic rounding (st_row4, common.cuh).
 #include "common.cuh"
 
 namespace dlrm {
@@ -23,7 +24,7 @@ constexpr int SMALL_CHUNK = 128;        // samples per accumulate CTA (512 would
 constexpr int SMALL_MAX_TABLES = 32;
 
 struct SmallTable {
-  float* w;
+  void* w;              // rows of the row type (float or __half)
   float* mom;
   const void* idx;
   const void* off;
@@ -46,6 +47,7 @@ struct SmallParams {
   float lr, eps;
   float* partial;       // [chunks][total small rows][dim]
   int total_rows, chunks;
+  unsigned long long round_key[SMALL_MAX_TABLES];   // fp16: stochastic-rounding key of table k for this step
 };
 
 __device__ __forceinline__ const float* small_dy_row(const SmallParams& P, long long bag) {
@@ -133,7 +135,7 @@ __global__ void __launch_bounds__(256) emb_small_accum_kernel(const __grid_const
     *reinterpret_cast<float4*>(dst + e) = *reinterpret_cast<const float4*>(acc + e);
 }
 
-template <int NV>
+template <typename wt, int NV>
 __global__ void __launch_bounds__(256) emb_small_apply_kernel(const __grid_constant__ SmallParams P, int num_tables) {
   const int lane = threadIdx.x & 31;
   const int grow = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);   // row in the partial row space
@@ -155,8 +157,10 @@ __global__ void __launch_bounds__(256) emb_small_apply_kernel(const __grid_const
         g[v].x += t.x; g[v].y += t.y; g[v].z += t.z; g[v].w += t.w;
       }
   }
-  float* wrow = tb.w + (long long)r * tb.ld + lane * 4;
+  wt* wrow = static_cast<wt*>(tb.w) + (long long)r * tb.ld + lane * 4;
   const float nlr = -P.lr;
+  unsigned long long rkey = 0;
+  if constexpr (is_f16<wt>::value) rkey = sr_row_key(P.round_key[k], r + tb.row_lo);
   if (P.optimizer == DLRM_OPT_RWSADAGRAD) {
     float sq = 0.f;
 #pragma unroll
@@ -170,20 +174,27 @@ __global__ void __launch_bounds__(256) emb_small_apply_kernel(const __grid_const
 #pragma unroll
     for (int v = 0; v < NV; ++v)
       if (lane * 4 + v * 128 < D) {
-        float4 w = *reinterpret_cast<float4*>(wrow + v * 128);
+        float4 w = ld_row4(wrow + v * 128);
         w.x = fmaf(nlr, g[v].x / stdv, w.x); w.y = fmaf(nlr, g[v].y / stdv, w.y);
         w.z = fmaf(nlr, g[v].z / stdv, w.z); w.w = fmaf(nlr, g[v].w / stdv, w.w);
-        *reinterpret_cast<float4*>(wrow + v * 128) = w;
+        st_row4(wrow + v * 128, w, is_f16<wt>::value ? sr_bits(rkey, lane + 32 * v) : 0ull);
       }
     if (lane == 0) tb.mom[(long long)r * tb.mom_stride] = m_new;
   } else {
+    if constexpr (is_f16<wt>::value) {      // untouched rows are not rewritten
+      bool nz = false;
+#pragma unroll
+      for (int v = 0; v < NV; ++v)
+        if (lane * 4 + v * 128 < D) nz = nz || g[v].x != 0.f || g[v].y != 0.f || g[v].z != 0.f || g[v].w != 0.f;
+      if (!__any_sync(0xffffffffu, nz)) return;
+    }
 #pragma unroll
     for (int v = 0; v < NV; ++v)
       if (lane * 4 + v * 128 < D) {
-        float4 w = *reinterpret_cast<float4*>(wrow + v * 128);
+        float4 w = ld_row4(wrow + v * 128);
         w.x = fmaf(nlr, g[v].x, w.x); w.y = fmaf(nlr, g[v].y, w.y);
         w.z = fmaf(nlr, g[v].z, w.z); w.w = fmaf(nlr, g[v].w, w.w);
-        *reinterpret_cast<float4*>(wrow + v * 128) = w;
+        st_row4(wrow + v * 128, w, is_f16<wt>::value ? sr_bits(rkey, lane + 32 * v) : 0ull);
       }
   }
 }
@@ -208,10 +219,15 @@ extern "C" int dlrm_b200_emb_bwd_small_update(const dlrm_emb_bwd_table_t* tables
   if (dim <= 0 || dim % 4 || dim > 512) return set_error("emb_bwd_small_update: dim=%d (multiple of 4, <= 512)", dim);
   if (!tables || !scratch || (!dY && !peer_dY)) return set_error("emb_bwd_small_update: NULL pointer");
   if (dy_stride_sample % 4) return set_error("emb_bwd_small_update: dY rows must be 16-byte aligned");
+  const int dtype = tables[0].weight_dtype;
+  if (dtype != DLRM_DTYPE_F32 && dtype != DLRM_DTYPE_F16) return set_error("emb_bwd_small_update: weight_dtype=%d", dtype);
+  if (dtype == DLRM_DTYPE_F16 && dim % 8) return set_error("emb_bwd_small_update: fp16 tables need dim %% 8 == 0 (dim=%d)", dim);
   SmallParams P{};
   int total_rows = 0, max_rows = 0;
   for (int k = 0; k < num_tables; ++k) {
     const dlrm_emb_bwd_table_t& s = tables[k];
+    if (s.weight_dtype != dtype)
+      return set_error("emb_bwd_small_update: table %d: weight_dtype differs from table 0's (one row type per call)", k);
     if (!s.weight || !s.offsets || (!s.indices && s.nnz > 0)) return set_error("emb_bwd_small_update: table %d NULL pointer", k);
     if (optimizer == DLRM_OPT_RWSADAGRAD && !s.momentum) return set_error("emb_bwd_small_update: table %d momentum NULL", k);
     const int64_t rn = s.row_n > 0 ? s.row_n : s.rows;
@@ -221,6 +237,7 @@ extern "C" int dlrm_b200_emb_bwd_small_update(const dlrm_emb_bwd_table_t* tables
     t.w = s.weight; t.mom = s.momentum; t.idx = s.indices; t.off = s.offsets; t.nnz = s.nnz;
     t.ld = s.ld > 0 ? s.ld : dim; t.mom_stride = s.mom_stride > 0 ? s.mom_stride : 1;
     t.dy_off = s.dy_off; t.row_lo = s.row_n > 0 ? s.row_lo : 0; t.row_n = (int)rn; t.part_row0 = total_rows;
+    P.round_key[k] = s.round_key;
     if (t.ld % 4 || (reinterpret_cast<uintptr_t>(t.w) & 15)) return set_error("emb_bwd_small_update: table %d rows not 16-byte aligned", k);
     total_rows += (int)rn;
     max_rows = (int)rn > max_rows ? (int)rn : max_rows;
@@ -251,7 +268,10 @@ extern "C" int dlrm_b200_emb_bwd_small_update(const dlrm_emb_bwd_table_t* tables
                                      200 * 1024));                                                                    \
     emb_small_accum_kernel<NV, IDX><<<dim3((unsigned)chunks, (unsigned)num_tables), 256, smem, st>>>(P);              \
     DLRM_CHECK_LAUNCH("emb_small_accum_kernel");                                                                      \
-    emb_small_apply_kernel<NV><<<(unsigned)((total_rows + 7) / 8), 256, 0, st>>>(P, num_tables);                      \
+    if (dtype == DLRM_DTYPE_F16)                                                                                      \
+      emb_small_apply_kernel<__half, NV><<<(unsigned)((total_rows + 7) / 8), 256, 0, st>>>(P, num_tables);            \
+    else                                                                                                              \
+      emb_small_apply_kernel<float, NV><<<(unsigned)((total_rows + 7) / 8), 256, 0, st>>>(P, num_tables);             \
     DLRM_CHECK_LAUNCH("emb_small_apply_kernel");                                                                      \
     return 0;                                                                                                         \
   } while (0)

@@ -54,13 +54,8 @@ __global__ void __launch_bounds__(256) block_copy_kernel(const __grid_constant__
     d[i] = s[i];
 }
 
-// ---- counter-based generator (mirror of dlrm_b200/mlperf.py: keep the two in sync, tests compare them bit for bit)
-__device__ __forceinline__ unsigned long long splitmix64(unsigned long long x) {
-  x += 0x9E3779B97F4A7C15ull;
-  x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
-  x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-  return x ^ (x >> 31);
-}
+// ---- counter-based generator (mirror of dlrm_b200/mlperf.py: keep the two in sync, tests compare them bit for bit;
+// splitmix64 is in common.cuh)
 constexpr unsigned long long K_TABLE = 0x9E3779B97F4A7C15ull, K_ROW = 0xC2B2AE3D27D4EB4Full,
                              K_SLOT = 0x165667B19E3779F9ull, K_STEP = 0xD6E8FEB86659FD93ull;
 

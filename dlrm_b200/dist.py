@@ -158,7 +158,9 @@ class DistEngine:
                                      % (self.Tg, self.world))
                 placement = P.contiguous(ln_emb, self.world)
             else:
-                placement = P.plan(ln_emb, cost if cost is not None else [1.0] * self.Tg, self.world)
+                # fp16 tables: the plan's memory budget counts their real row size (fp32 keeps the plan's default)
+                pkw = {"bytes_per_row": P.row_bytes(m_spa, "fp16")} if kw.get("emb_dtype") == "fp16" else {}
+                placement = P.plan(ln_emb, cost if cost is not None else [1.0] * self.Tg, self.world, **pkw)
         self.pl = placement
         if exchange == "nccl" and (self.pl.split_tables() or
                                    [(s.table, s.rank) for s in sorted(self.pl.shards, key=lambda s: s.table)] !=
@@ -309,7 +311,7 @@ class DistEngine:
             for s in sh:
                 own = self.pl.of_rank(s.rank)
                 row0 = sum(o.local_rows for o in own[:own.index(s)])       # rows before shard s in the owner's arena
-                bases.append(ptrs[s.rank][0] + row0 * e.ldw * 4)
+                bases.append(ptrs[s.rank][0] + row0 * e.ldw * e.esize)
             tabs[t] = (bases, sh[0].local_rows)
         e.use_remote_reads(tabs)
         e.remote_sample0 = self.rank * self.B
@@ -398,7 +400,7 @@ class DistEngine:
             nsplit = sum(1 for s in self.mine if not s.whole)               # no partial sums pushed, rows PULLED instead
             fwd -= nsplit * self.Bg * D * 4 * remote
             if lookups is not None:
-                rd = sum(float(lookups[t]) for t in self.pl.split_tables()) * B * D * 4 * remote
+                rd = sum(float(lookups[t]) for t in self.pl.split_tables()) * B * D * self.eng.esize * remote
         bwd = sum(sum(1 for s in self.pl.of_table(t) if s.rank != self.rank) for t in range(self.Tg)) * B * D * 4
         idx = staged_index_bytes * remote                                    # upper bound: split tables go to every rank
         tot = fwd + bwd + idx + rd
@@ -411,7 +413,7 @@ class DistEngine:
         ld = 0.0
         for s in self.mine:
             ld += float(lookups_per_sample[s.table]) * (s.local_rows / max(s.rows, 1))
-        return ld * self.Bg * self.D * 4
+        return ld * self.Bg * self.D * self.eng.esize
 
 
 # ---------------------------------------------------------------------------- fixed-length (multi-hot) inputs

@@ -15,7 +15,10 @@ Parameters are VIEWS into the engine's HBM arenas (one table arena, one dense ar
 one autograd node whose backward runs the engine's backward kernels.  Embedding gradients are either
   - handed to a fused optimizer of `dlrm_b200.optim` (no [nnz, D] gradient is ever materialised), or
   - materialised as the reference's uncoalesced sparse COO tensors (`emb_l[k].weight.grad`) so an
-    unmodified `torch.optim.SGD` keeps working (compatibility mode, slower).
+    unmodified `torch.optim.SGD` keeps working (compatibility mode, slower; fp32 tables only).
+`emb_dtype=torch.float16` stores the tables as fp16 (`emb_l[k].weight` is an fp16 strided parameter): lookups widen
+the rows to fp32, the fused optimizers update them in fp32 and store them with stochastic rounding.  `state_dict()`
+then holds fp16 tables; an fp32 checkpoint loads with round-to-nearest, an fp16 one into an fp32 model exactly.
 QR / mixed-dimension embeddings, quantised embeddings and `parallel_forward` are outside the path
 (SURVEY §2) and exit with an error when requested.
 """
@@ -33,6 +36,14 @@ from .engine import Engine, SparseInput, sparse_from_reference
 # Above this many table elements the reference's numpy initialisation (one np.random.uniform call per
 # table, 150 s for 26 x 1e6 x 128) is replaced by the same distribution drawn on the device.
 _NUMPY_INIT_MAX = 50_000_000
+
+
+def _uniform_(tab: torch.Tensor, a: float, gen):
+    """U(-a, a) drawn in fp32 on the device (fp16 tables: that draw rounded to nearest)."""
+    if tab.dtype == torch.float32:
+        tab.uniform_(-a, a, generator=gen)
+    else:
+        tab.copy_(torch.empty(tab.shape, dtype=torch.float32, device=tab.device).uniform_(-a, a, generator=gen))
 
 
 class _TableView(nn.Module):
@@ -81,6 +92,9 @@ class _DLRMForward(torch.autograd.Function):
         net, eng = ctx.net, ctx.net._engine
         eng.backward_from_output_grad(ctx.x, ctx.sp, gp.contiguous())
         grads: List[Optional[torch.Tensor]] = []
+        if net._fused_opt is None and eng.f16:
+            raise RuntimeError("dlrm_b200: fp16 embedding tables are trained by the fused optimizers of "
+                               "dlrm_b200.optim (SGD, RWSAdagrad); create one before calling backward()")
         if net._fused_opt is not None:
             if net._pending is not None:
                 raise RuntimeError("dlrm_b200: backward() called twice before optimizer.step(): gradient "
@@ -101,7 +115,8 @@ class DLRM_Net(nn.Module):
                  arch_interaction_itself=False, sigmoid_bot=-1, sigmoid_top=-1, sync_dense_params=True,
                  loss_threshold=0.0, ndevices=-1, qr_flag=False, qr_operation="mult", qr_collisions=0,
                  qr_threshold=200, md_flag=False, md_threshold=200, weighted_pooling=None,
-                 loss_function="bce", *, device=None, gemm="tc", max_batch=2048, loss_weights=None):
+                 loss_function="bce", *, device=None, gemm="tc", max_batch=2048, loss_weights=None,
+                 emb_dtype=torch.float32, round_seed=0):
         super().__init__()
         self._engine: Optional[Engine] = None
         self._fused_opt = None
@@ -109,6 +124,14 @@ class DLRM_Net(nn.Module):
         if (m_spa is None or ln_emb is None or ln_bot is None or ln_top is None
                 or arch_interaction_op is None):
             return  # reference allows an empty shell (dlrm_s_pytorch.py:320-326)
+        if emb_dtype in (torch.float16, "fp16", "float16"):
+            emb_dtype = "fp16"
+        elif emb_dtype in (torch.float32, "fp32", "float32"):
+            emb_dtype = "fp32"
+        else:
+            sys.exit("ERROR: emb_dtype must be torch.float32 or torch.float16")
+        if emb_dtype == "fp16" and int(m_spa) % 8:
+            sys.exit("ERROR: fp16 embedding tables need an embedding dimension divisible by 8")
         if qr_flag or md_flag:
             sys.exit("ERROR: --qr-flag / --md-flag embeddings are outside the dlrm_b200 hot path")
         if arch_interaction_op not in ("dot", "cat"):
@@ -156,7 +179,8 @@ class DLRM_Net(nn.Module):
             self._dist = DistEngine(int(m_spa), ln_emb.tolist(), ln_bot.tolist(), ln_top.tolist(),
                                     local_batch=max_batch // world, device=device, gemm=gemm, loss=loss_function,
                                     exchange="p2p", itself=arch_interaction_itself, sigmoid_bot=sigmoid_bot,
-                                    loss_threshold=loss_threshold, loss_ws=loss_ws)
+                                    loss_threshold=loss_threshold, loss_ws=loss_ws, emb_dtype=emb_dtype,
+                                    round_seed=round_seed)
             self._engine = self._dist.eng
             self.local_shards = list(self._dist.mine)
         else:
@@ -164,7 +188,8 @@ class DLRM_Net(nn.Module):
                                   op=arch_interaction_op, itself=arch_interaction_itself,
                                   sigmoid_bot=sigmoid_bot, sigmoid_top=sigmoid_top, loss=loss_function,
                                   loss_threshold=loss_threshold, loss_ws=loss_ws, device=device,
-                                  max_batch=max_batch, gemm=gemm, interleave_momentum=False)
+                                  max_batch=max_batch, gemm=gemm, emb_dtype=emb_dtype, round_seed=round_seed,
+                                  interleave_momentum=None if emb_dtype == "fp16" else False)
         self._m_spa, self._ln_emb = int(m_spa), ln_emb
         # same construction (and numpy RNG consumption) order as the reference: tables, bottom, top
         if ndevices <= 1:
@@ -234,7 +259,7 @@ class DLRM_Net(nn.Module):
                     tab = eng.table(j)
                     with torch.no_grad():
                         if big:
-                            tab.uniform_(-a, a, generator=gen)
+                            _uniform_(tab, a, gen)
                         else:
                             tab.copy_(torch.from_numpy(W[lo:lo + cnt]))
                     views[j] = _TableView(tab)
@@ -248,7 +273,7 @@ class DLRM_Net(nn.Module):
             a = float(np.sqrt(1 / n))
             with torch.no_grad():
                 if big:
-                    tab.uniform_(-a, a, generator=gen)
+                    _uniform_(tab, a, gen)
                 else:  # bit-identical to the reference for the same numpy seed (dlrm_s_pytorch.py:280-284)
                     W = np.random.uniform(low=-a, high=a, size=(n, int(m))).astype(np.float32)
                     tab.copy_(torch.from_numpy(W))

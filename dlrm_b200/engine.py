@@ -12,6 +12,7 @@ libdlrm_b200.so.  No CPU fallback exists: a missing library or device raises.
 
 HBM layout (fp32 unless noted)
   tables   [sum_k rows_k, D]   one allocation; table k = rows [row_base_k, row_base_k + rows_k)
+                               (emb_dtype="fp16": fp16 rows [D halves | fp32 accumulator | int32 head | pad])
   momentum [sum_k rows_k]      RWSAdagrad row-wise accumulator (optim/rwsadagrad.py:91-95)
   head     [sum_k rows_k] i32  per-row list heads for the sort-free coalesce (zero between steps)
   mark     [nnz] u8            per-occurrence superseded marks beside link[] (zero between steps)
@@ -32,8 +33,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import (ACT_NONE, ACT_RELU, ACT_SIGMOID, GEMM_SIMT_FP32, LOSS_BCE, LOSS_MSE, LOSS_WBCE,
-                   OPT_RWSADAGRAD, OPT_SGD, EmbBwdTable, EmbFwdTable)
+from ._lib import (ACT_NONE, ACT_RELU, ACT_SIGMOID, DTYPE_F16, DTYPE_F32, GEMM_SIMT_FP32, LOSS_BCE, LOSS_MSE,
+                   LOSS_WBCE, OPT_RWSADAGRAD, OPT_SGD, EmbBwdTable, EmbFwdTable)
 
 _LOSS = {"mse": LOSS_MSE, "bce": LOSS_BCE, "wbce": LOSS_WBCE}
 _OPT = {"sgd": OPT_SGD, "rwsadagrad": OPT_RWSADAGRAD}
@@ -45,6 +46,28 @@ def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
 
 def _stream() -> int:
     return torch.cuda.current_stream().cuda_stream
+
+
+_M64 = (1 << 64) - 1
+
+
+def _splitmix64(x: int) -> int:
+    x = (x + 0x9E3779B97F4A7C15) & _M64
+    x = ((x ^ (x >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    x = ((x ^ (x >> 27)) * 0x94D049BB133111EB) & _M64
+    return x ^ (x >> 31)
+
+
+def round_key(seed: int, step: int, table: int) -> int:
+    """Stochastic-rounding key of a global table at optimizer step `step` (dlrm_emb_bwd_table_t.round_key): the hash
+    prefix of (seed, step, table), keyed like the synthetic batches of mlperf.py."""
+    base = ((seed * 0xD6E8FEB86659FD93) ^ ((step + 1) * 0x9E3779B97F4A7C15) ^ ((table + 1) * 0x165667B19E3779F9)) & _M64
+    return _splitmix64(base)
+
+
+def fp16_row_stride(dim: int) -> int:
+    """Row stride (halves) of an fp16 table row [dim halves | fp32 accumulator | int32 head | pad], 16-byte aligned."""
+    return (2 * dim + 8 + 15) // 16 * 16 // 2
 
 
 @dataclass
@@ -73,7 +96,8 @@ class Engine:
                  *, op: str = "dot", itself: bool = False, sigmoid_bot: int = -1, sigmoid_top: int = -1,
                  loss: str = "bce", loss_threshold: float = 0.0, loss_ws=None, device="cuda:0",
                  max_batch: int = 2048, gemm: str = "simt", n_features: Optional[int] = None,
-                 interleave_momentum: Optional[bool] = None, shards=None, split_slots=None, small_rows_max: int = 256):
+                 interleave_momentum: Optional[bool] = None, shards=None, split_slots=None, small_rows_max: int = 256,
+                 emb_dtype: str = "fp32", round_seed: int = 0):
         if not torch.cuda.is_available():
             raise RuntimeError("dlrm_b200.Engine needs a CUDA device (H100, sm_90a); there is no CPU path")
         self.device = torch.device(device)
@@ -132,6 +156,19 @@ class Engine:
             raise ValueError("# of feature interactions %d does not match first dimension of top mlp %d"
                              % (self.num_int, self.ln_top[0]))
         dev = self.device
+        # ---- table row type.  fp16: rows are stored as IEEE halves, widened to fp32 by the gather and the update, and
+        # written back with stochastic rounding keyed by (round_seed, opt_step, global table, global row, column).
+        if emb_dtype not in ("fp32", "fp16"):
+            raise ValueError("emb_dtype must be fp32 or fp16")
+        self.emb_dtype = emb_dtype
+        self.f16 = emb_dtype == "fp16"
+        self.round_seed = int(round_seed)
+        self.wdtype = torch.float16 if self.f16 else torch.float32
+        self.esize = 2 if self.f16 else 4          # bytes per stored table element
+        if self.f16 and self.D % 8:
+            raise ValueError("fp16 embedding tables need a dimension divisible by 8 (got %d)" % self.D)
+        if self.f16 and interleave_momentum is False:
+            raise ValueError("fp16 embedding tables always keep the accumulator and list head inside the row")
         # ---- tables
         rows = np.asarray(self.ln_emb, dtype=np.int64)
         self.row_base = np.concatenate([[0], np.cumsum(rows)]).astype(np.int64)
@@ -143,13 +180,15 @@ class Engine:
         # row.  The gather pays a little bandwidth for rows that are no longer 512-byte aligned (528-byte stride).
         # interleave=False: dense [rows, D] tables + separate accumulator / head arrays (round 1's layout).
         if interleave_momentum is None:
-            interleave_momentum = (self.D % 4 == 0) and os.environ.get("DLRM_ROW_META", "1") != "0"
+            interleave_momentum = self.f16 or ((self.D % 4 == 0) and os.environ.get("DLRM_ROW_META", "1") != "0")
         self.interleave = bool(interleave_momentum)
         # DLRM_ROW_PAD: floats appended to a row (>= 2: accumulator + list head).  4 keeps rows 16-B aligned (+3 % memory);
         # 16 keeps 512-B rows 64-B aligned (every row the same 8 DRAM atoms + 1 for the two words, +12.5 % memory).
         self.row_pad = max(4, (int(os.environ.get("DLRM_ROW_PAD", "4")) + 3) // 4 * 4)
-        self.ldw = self.D + self.row_pad if self.interleave else self.D
-        self.tables = torch.zeros((self.total_rows, self.ldw), dtype=torch.float32, device=dev)
+        self.ldw = self.D + self.row_pad if self.interleave else self.D        # row stride in stored elements
+        if self.f16:
+            self.ldw = fp16_row_stride(self.D)      # D + 8 halves at D % 8 == 0: 272 bytes at D = 128
+        self.tables = torch.zeros((self.total_rows, self.ldw), dtype=self.wdtype, device=dev)
         self._head_sep = None if self.interleave else torch.zeros(self.total_rows, dtype=torch.int32, device=dev)
         self._momentum_sep: Optional[torch.Tensor] = None
         self.row_weights: Optional[torch.Tensor] = None  # weighted pooling v_W_l, arena [total_rows]
@@ -278,6 +317,7 @@ class Engine:
             for i, p_ in enumerate(ptrs):
                 d.shard_weight[i] = p_
             d.num_shards, d.rows_per_shard, d.rows, d.ld = len(ptrs), int(rps), int(self.shards[k]["rows"]), self.ldw
+            d.weight_dtype = DTYPE_F16 if self.f16 else DTYPE_F32
             es = sp.offsets[k].element_size()
             d.indices = sp.indices[k].data_ptr() if sp.indices[k].numel() else 0
             d.offsets = sp.offsets[k].data_ptr() + self.remote_sample0 * es     # my bags inside the global stream
@@ -308,7 +348,7 @@ class Engine:
             tables = {}
             for t, n in self.split_slots:
                 js = sorted((int(sh["part"]), j) for j, sh in enumerate(self.shards) if int(sh["table"]) == t)
-                ptrs = [self.tables.data_ptr() + int(self.row_base[j]) * self.ldw * 4 for _, j in js]
+                ptrs = [self.tables.data_ptr() + int(self.row_base[j]) * self.ldw * self.esize for _, j in js]
                 rps = int(self.shards[js[0][1]]["row_n"])
                 tables[t] = (ptrs, rps)
         self.remote_tables = tables
@@ -344,18 +384,23 @@ class Engine:
         self._filtered = False
 
     def table(self, k: int) -> torch.Tensor:
-        """[rows_k, D] view of table k (strided when the accumulator is interleaved)."""
+        """[rows_k, D] view of table k (strided when the accumulator is interleaved; fp16 with emb_dtype="fp16")."""
         return self.tables[int(self.row_base[k]):int(self.row_base[k + 1]), :self.D]
+
+    @property
+    def _meta_col(self) -> int:
+        """Column of the accumulator in the 4-byte view of an interleaved row (the list head is the next one)."""
+        return self.D * self.esize // 4
 
     @property
     def head(self) -> torch.Tensor:
         """Per-row list heads of the sort-free coalesce, [sum rows] int32 (a strided view when interleaved)."""
-        return self.tables.view(torch.int32)[:, self.D + 1] if self.interleave else self._head_sep
+        return self.tables.view(torch.int32)[:, self._meta_col + 1] if self.interleave else self._head_sep
 
     @property
     def momentum(self) -> Optional[torch.Tensor]:
-        """Row-wise Adagrad accumulator of every row, [sum rows] (a strided view when interleaved)."""
-        return self.tables[:, self.D] if self.interleave else self._momentum_sep
+        """Row-wise Adagrad accumulator of every row, [sum rows] fp32 (a strided view when interleaved)."""
+        return self.tables.view(torch.float32)[:, self._meta_col] if self.interleave else self._momentum_sep
 
     def ensure_optimizer_state(self, optimizer: str):
         if optimizer == "rwsadagrad":
@@ -374,7 +419,7 @@ class Engine:
         """params = dict(emb=[W_k], bot=[(W,b)...], top=[(W,b)...], v_W_l=None|[...]) of numpy /
         torch arrays (the layout of the oracle and of the reference's state_dict)."""
         with torch.no_grad():
-            for k, Wk in enumerate(params["emb"]):
+            for k, Wk in enumerate(params["emb"]):     # fp16 tables: round to nearest
                 self.table(k).copy_(torch.as_tensor(Wk, dtype=torch.float32))
             for name in ("bot", "top"):
                 for i, (Wl, bl) in enumerate(params[name]):
@@ -392,12 +437,24 @@ class Engine:
         self._pack_dirty = True
         g = torch.Generator(device=self.device)
         g.manual_seed(seed)
+        # row stride of an fp32 engine built with the same arguments (its default layout): fp16 tables draw like it
+        ld32 = self.D + self.row_pad if (self.D % 4 == 0 and os.environ.get("DLRM_ROW_META", "1") != "0") else self.D
         with torch.no_grad():
             for k, n in enumerate(self.ln_emb):
                 a = float(np.sqrt(1.0 / int(self.shards[k]["rows"])))      # the bound of the WHOLE table (:280-284)
                 tk = self.table(k)
-                for r0 in range(0, tk.shape[0], 1 << 24):                    # chunks: any temporary stays < 8.6 GB
-                    tk[r0:r0 + (1 << 24)].uniform_(-a, a, generator=g)
+                for r0 in range(0, tk.shape[0], 1 << 24):                    # chunks: any temporary stays < 9 GB
+                    if self.f16:
+                        # the fp32 draw of an fp32 engine, rounded to nearest.  The draw goes into a view with the
+                        # fp32 engine's sizes AND row stride: torch's generator maps values to elements through the
+                        # iteration space of its output (split into 32-bit-indexable pieces by the byte span), so
+                        # only an identical view draws identical values.
+                        n = tk[r0:r0 + (1 << 24)].shape[0]
+                        tmp = torch.empty((n, ld32), dtype=torch.float32, device=self.device)[:, :self.D]
+                        tk[r0:r0 + (1 << 24)].copy_(tmp.uniform_(-a, a, generator=g))
+                        del tmp
+                    else:
+                        tk[r0:r0 + (1 << 24)].uniform_(-a, a, generator=g)
             for name, ln in (("bot", self.ln_bot), ("top", self.ln_top)):
                 for i in range(len(ln) - 1):
                     n, m = ln[i], ln[i + 1]
@@ -412,8 +469,9 @@ class Engine:
         for n, k in enumerate(ks):
             d = arr[n]
             sh = self.shards[k]
-            d.weight = self.tables.data_ptr() + int(self.row_base[k]) * self.ldw * 4
+            d.weight = self.tables.data_ptr() + int(self.row_base[k]) * self.ldw * self.esize
             d.ld = self.ldw
+            d.weight_dtype = DTYPE_F16 if self.f16 else DTYPE_F32
             d.indices = sp.indices[k].data_ptr() if sp.indices[k].numel() else 0
             d.offsets = sp.offsets[k].data_ptr()
             d.row_weights = (self.row_weights.data_ptr() + int(self.row_base[k]) * 4
@@ -435,11 +493,14 @@ class Engine:
             d.row_lo, d.row_n = int(sh["row_lo"]), int(sh["row_n"])
             if dy_off is not None:
                 d.use_dy_off, d.dy_off = 1, int(dy_off[k])
-            d.weight = self.tables.data_ptr() + int(self.row_base[k]) * self.ldw * 4
+            d.weight = self.tables.data_ptr() + int(self.row_base[k]) * self.ldw * self.esize
             d.ld = self.ldw
+            if self.f16:
+                d.weight_dtype = DTYPE_F16
+                d.round_key = round_key(self.round_seed, self.opt_step, int(sh["table"]))
             if self.interleave:
-                d.momentum = d.weight + self.D * 4
-                d.mom_stride = self.ldw
+                d.momentum = d.weight + self.D * self.esize
+                d.mom_stride = self.ldw * self.esize // 4
             else:
                 d.momentum = (self._momentum_sep.data_ptr() + int(self.row_base[k]) * 4
                               if self._momentum_sep is not None else None)
@@ -448,7 +509,7 @@ class Engine:
             if self.is_small(k):
                 d.head = None
             elif self.interleave:
-                d.head, d.head_stride = d.weight + (self.D + 1) * 4, self.ldw
+                d.head, d.head_stride = d.weight + self.D * self.esize + 4, self.ldw * self.esize // 4
             else:
                 d.head, d.head_stride = self._head_sep.data_ptr() + int(self.row_base[k]) * 4, 1
             d.mark = self.mark.data_ptr() if self.mark is not None else None
@@ -1322,12 +1383,21 @@ class Engine:
                 self._mark("join_update")
 
 
+def _refuse_graphed_f16(eng: "Engine"):
+    # The stochastic-rounding key of an fp16 table depends on the optimizer step and travels in the update's launch
+    # parameters: a replayed graph would round every step with the bits of the captured one.
+    if eng.f16:
+        raise RuntimeError("fp16 embedding tables train with eager steps: a captured training step would replay one "
+                           "step's stochastic-rounding bits on every replay")
+
+
 class GraphedTrainSteps:
     """K consecutive training steps over K static batch buffers in ONE CUDA graph.  Inside the graph
     the embedding update of step j overlaps the bottom MLP of step j+1 (train_step(join_update=False));
     only the last update is joined.  `losses[j]` holds the loss of step j after a replay."""
 
     def __init__(self, eng: "Engine", stages, lr: float, optimizer: str = "rwsadagrad", warmup: int = 2):
+        _refuse_graphed_f16(eng)
         self.eng, self.stages, self.lr, self.optimizer = eng, list(stages), lr, optimizer
         self.K = len(self.stages)
         eng.ensure_optimizer_state(optimizer)
@@ -1369,6 +1439,8 @@ class GraphedTrainStep:
                  train: bool = True, X: Optional[torch.Tensor] = None, target: Optional[torch.Tensor] = None,
                  pre=None):
         """pre: optional callable run (and captured) before the step, e.g. the index exchange of a sharded run."""
+        if train:
+            _refuse_graphed_f16(eng)
         self.eng, self.stage, self.train, self.pre = eng, stage, train, pre
         # table-wise sharded runs: the dense slice / targets are separate static tensors
         self.X = X if X is not None else stage.X

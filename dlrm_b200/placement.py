@@ -84,6 +84,17 @@ def contiguous(rows: Sequence[int], world: int) -> Placement:
     return Placement(world, shards, [1.0] * T)
 
 
+def row_bytes(dim: int, emb_dtype: str = "fp32") -> int:
+    """Bytes a table row takes in HBM: an fp32 row counted as its weights (dim * 4; `plan` defaults to 512, the
+    dim-128 value); an fp16 row is its halves plus the fp32 accumulator and int32 list head, padded to 16 bytes
+    (272 bytes at dim 128)."""
+    if emb_dtype == "fp16":
+        return (2 * int(dim) + 8 + 15) // 16 * 16
+    if emb_dtype == "fp32":
+        return 4 * int(dim)
+    raise ValueError("emb_dtype must be fp32 or fp16")
+
+
 def plan(rows: Sequence[int], cost: Sequence[float], world: int, *, split_above: float = 0.6,
          bytes_per_row: int = 512, mem_budget_bytes: float = 150e9, force_split: Sequence[int] = (),
          target_imbalance: float = 1.06, max_extra_splits: int = 4) -> Placement:

@@ -20,6 +20,11 @@
  *   - float = IEEE fp32.  Index/offset tensors are int64 (idx_bytes=8) or int32
  *     (idx_bytes=4), both arrays of one call having the same width, exactly as
  *     nn.EmbeddingBag accepts them; they are consumed bit-for-bit, never copied.
+ *   - Embedding tables are fp32 or IEEE fp16 (weight_dtype, DLRM_DTYPE_*; all tables of one call
+ *     share it).  fp16 rows are widened to fp32 for every sum and every optimizer step; the row-wise
+ *     accumulator, the list head and all arithmetic stay fp32 / int32.  The `weight` fields keep their
+ *     float* type and then point at halves; `ld` always counts elements of the row type.  fp16 needs
+ *     dim % 8 == 0.  A zero-initialised descriptor means fp32.
  */
 #ifndef DLRM_B200_H_
 #define DLRM_B200_H_
@@ -43,6 +48,8 @@ enum { DLRM_LOSS_MSE = 0, DLRM_LOSS_BCE = 1, DLRM_LOSS_WBCE = 2 };
 enum { DLRM_OPT_SGD = 0, DLRM_OPT_RWSADAGRAD = 1 };
 /* GEMM back ends */
 enum { DLRM_GEMM_SIMT_FP32 = 0, DLRM_GEMM_TC_BF16X3 = 1, DLRM_GEMM_TC_BF16 = 2 };
+/* storage type of embedding table rows (weight_dtype of the table descriptors) */
+enum { DLRM_DTYPE_F32 = 0, DLRM_DTYPE_F16 = 1 };
 
 int dlrm_b200_abi_version(void);
 const char* dlrm_b200_last_error(void);
@@ -65,14 +72,14 @@ int dlrm_b200_set_tunable(int id, int value);
  * offsets has batch+1 entries and `nnz` is ignored (graph-replay friendly).  Empty bag -> 0.
  * ------------------------------------------------------------------------------------------ */
 typedef struct {
-  const float* weight;      /* [rows, dim] row-major, 16-byte aligned when dim % 4 == 0 */
+  const float* weight;      /* [rows, dim] row-major (fp32, or fp16 per weight_dtype), 16-byte aligned when dim % 4 == 0 */
   const void* indices;      /* [nnz]   int64 / int32 */
   const void* offsets;      /* [batch] (or [batch+1] when include_last) same type */
   const float* row_weights; /* NULL, or [rows]: v_W_l[k] (weighted pooling, :425-428) */
   int64_t nnz;
   int64_t rows;             /* rows of the WHOLE table: an index outside [0, rows) sets the device error word
                              * (dlrm_b200_check_device_errors) and is read as row 0 / skipped; 0 = unchecked */
-  int64_t ld;               /* row stride of `weight` in floats; 0 = dim (dense rows) */
+  int64_t ld;               /* row stride of `weight` in elements of the row type; 0 = dim (dense rows) */
   /* Sharded placement (dlrm_b200/placement.py).  All zero = the call-level layout out[b, k, :].
    * out_stride > 0: the pooled row of bag b goes to out (or the owner's peer buffer) + b_local*out_stride + out_off
    *   -- a whole table lands in feature slot 1+t of the interaction operand, a row-split shard in its slab of
@@ -81,6 +88,8 @@ typedef struct {
    *   to another shard and are skipped (a partial sum over this shard's rows). */
   int64_t out_off, out_stride;
   int64_t row_lo, row_n;
+  int32_t weight_dtype;     /* DLRM_DTYPE_F32 (0) or DLRM_DTYPE_F16: fp16 rows are widened to fp32 and summed as above,
+                             * so the pooled output equals the fp32 gather over the widened table bit for bit */
 } dlrm_emb_fwd_table_t;
 
 int dlrm_b200_emb_bag_fwd(const dlrm_emb_fwd_table_t* tables /*[host]*/, int num_tables, int dim,
@@ -106,6 +115,13 @@ int dlrm_b200_emb_bag_fwd(const dlrm_emb_fwd_table_t* tables /*[host]*/, int num
  *   RWSAdagrad: momentum[row] += mean_d(g^2); W[row] -= lr * g / (sqrt(momentum[row]) + eps)
  *   SGD:        W[row] -= lr * g
  * `lr` is the already-decayed clr of optim/rwsadagrad.py:115.
+ * fp16 tables (weight_dtype = DLRM_DTYPE_F16): the row is widened to fp32, the step above runs in fp32 with the
+ * operations of the fp32 kernel, and the result x is stored with STOCHASTIC ROUNDING: x itself when it is an
+ * fp16 value, else lo (the fp16 neighbour toward zero) or hi (the one away from zero), hi iff
+ *   r < floor(2^16 * (|x| - |lo|) / (|hi| - |lo|)),
+ * |x| > 65504 -> +-inf, NaN stays NaN.  r = 16 bits of h = splitmix64(round_key ^ R * 0xC2B2AE3D27D4EB4F ^
+ * (c / 4) * 0x165667B19E3779F9) for global row R = row_lo + local row and column c: bits [16 (c % 4), +16) of h.
+ * Rows that are not updated are not rewritten.
  * dY[b, k, :] is read at dY + b*dy_stride_sample + k*dy_stride_table.
  * ------------------------------------------------------------------------------------------ */
 typedef struct {
@@ -117,7 +133,9 @@ typedef struct {
   int64_t nnz;
   int64_t rows;
   int64_t pair_base;    /* first slot of this table in next[] / (sum of nnz of earlier tables) */
-  int64_t ld;           /* row stride of `weight` in floats; 0 = dim */
+  int64_t ld;           /* row stride of `weight` in elements of the row type; 0 = dim.  fp16: the weight pointer
+                         * 16-byte aligned and ld % 4 == 0 (rows on 8-byte boundaries); ld % 8 == 0 (16-byte rows, the
+                         * engine's layout) lets dim <= 128 take the faster kernel with one 16-byte access per lane */
   int64_t mom_stride;   /* elements between consecutive rows' accumulators in `momentum`; 0 = 1.
                          * ld = dim + 4 with momentum = weight + dim and mom_stride = ld keeps the
                          * row-wise Adagrad accumulator in the SAME DRAM burst as its row: the update then
@@ -139,6 +157,12 @@ typedef struct {
    * the same row was linked.  Zero-initialised scratch, all zero between steps (the update clears what the
    * link set).  Required whenever head != NULL. */
   uint8_t* mark;
+  /* DLRM_DTYPE_F32 (0) or DLRM_DTYPE_F16 (weight points at halves; ld in halves; momentum / head keep their own
+   * fp32 / int32 strides -- the interleaved fp16 row is [dim halves | fp32 accumulator | int32 head | pad]). */
+  int32_t weight_dtype;
+  /* fp16 only: stochastic-rounding key of this table for this step (see above), the hash prefix
+   * splitmix64(seed * 0xD6E8FEB86659FD93 ^ (step + 1) * 0x9E3779B97F4A7C15 ^ (global table + 1) * 0x165667B19E3779F9) */
+  uint64_t round_key;
 } dlrm_emb_bwd_table_t;
 
 /* Optional duplicate filter (dlrm_emb_dedup_t): at 1e6-row tables almost every row of a batch is
@@ -412,6 +436,7 @@ typedef struct {
   int64_t ld;
   const void* indices; const void* offsets; int64_t nnz;
   int64_t out_off, out_stride;
+  int32_t weight_dtype;     /* DLRM_DTYPE_F32 (0) or DLRM_DTYPE_F16; ld in elements of the row type */
 } dlrm_emb_remote_table_t;
 int dlrm_b200_emb_bag_fwd_remote(const dlrm_emb_remote_table_t* tables /*[host]*/, int num_tables, int dim,
                                  int64_t batch, int idx_bytes, int include_last, float* out, void* stream);
