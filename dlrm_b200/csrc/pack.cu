@@ -55,12 +55,15 @@ __global__ void __launch_bounds__(256) dense_update_pack_kernel(const __grid_con
     const int n = (int)(e / K1), k = (int)(e - (unsigned)n * K1);
     const bool is_b = k == L.K;
     const long long o = is_b ? n : (long long)n * L.K + k;
-    const float* gp = is_b ? L.db : L.dW;
-    float g = gp[o];
-    for (int s = 1; s < L.nslabs; ++s) g += gp[o + s * L.slab_stride];  // fixed order: deterministic
-    if (P.optimizer == -2) {  // fold the slabs only (the caller all-reduces slab 0 next)
-      const_cast<float*>(gp)[o] = g;
-      return;
+    float g = 0.f;
+    if (P.optimizer >= 0 || P.optimizer == -2) {  // pack only (-1) reads no gradient: dW / db may be NULL
+      const float* gp = is_b ? L.db : L.dW;
+      g = gp[o];
+      for (int s = 1; s < L.nslabs; ++s) g += gp[o + s * L.slab_stride];  // fixed order: deterministic
+      if (P.optimizer == -2) {  // fold the slabs only (the caller all-reduces slab 0 next)
+        const_cast<float*>(gp)[o] = g;
+        return;
+      }
     }
     float* pp = is_b ? L.b : L.W;
     float p = pp[o];
@@ -101,7 +104,7 @@ extern "C" int dlrm_b200_dense_update_pack(const dlrm_dense_layer_t* layers, int
   using namespace dlrm;
   if (num_layers <= 0) return 0;
   if (num_layers > 16) return set_error("dense_update_pack: at most 16 layers per call (got %d)", num_layers);
-  if (optimizer > DLRM_OPT_RWSADAGRAD) return set_error("dense_update_pack: optimizer=%d", optimizer);
+  if (optimizer < -2 || optimizer > DLRM_OPT_RWSADAGRAD) return set_error("dense_update_pack: optimizer=%d", optimizer);
   DenseLayers P;
   long long ctas = 0;
   for (int i = 0; i < num_layers; ++i) {
