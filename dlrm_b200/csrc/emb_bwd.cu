@@ -318,8 +318,10 @@ __global__ void __launch_bounds__(256) emb_classify_kernel(const __grid_constant
     const int kk = table_of(bound, num_tables, pos < total ? pos : first);
     if (pos < total && pos < tend[kk]) {
       const EmbBwdTable& tb = P.t[kk];
-      const long long r = static_cast<const idx_t*>(tb.idx)[pos - tb.pair_base];
-      susp = filter[filter_slot(tb.head + r * tb.hs, log2_size)] > 1u;
+      // local row, as the gather counted it; rows of another shard and tables without lists are never linked
+      const long long r = (long long)static_cast<const idx_t*>(tb.idx)[pos - tb.pair_base] - tb.row_lo;
+      if (tb.head != nullptr && (unsigned long long)r < (unsigned long long)tb.row_n)
+        susp = filter[filter_slot(tb.head + r * tb.hs, log2_size)] > 1u;
       flags[pos] = susp ? 1 : 0;
     }
     const unsigned m = __ballot_sync(0xffffffffu, susp);
@@ -343,7 +345,7 @@ __global__ void __launch_bounds__(256) emb_link_suspects_kernel(const __grid_con
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const long long pos = suspects[i];
     const EmbBwdTable& tb = P.t[table_of(bound, num_tables, pos)];
-    const long long r = static_cast<const idx_t*>(tb.idx)[pos - tb.pair_base];
+    const long long r = (long long)static_cast<const idx_t*>(tb.idx)[pos - tb.pair_base] - tb.row_lo;   // in range: classify
     const int prev = atomicExch(tb.head + r * tb.hs, (int)(pos + 1));
     P.link[pos].x = prev;
     if (prev) tb.mark[prev - 1] = 1;

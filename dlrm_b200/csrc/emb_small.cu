@@ -161,14 +161,21 @@ __global__ void __launch_bounds__(256) emb_small_apply_kernel(const __grid_const
   const float nlr = -P.lr;
   unsigned long long rkey = 0;
   if constexpr (is_f16<wt>::value) rkey = sr_row_key(P.round_key[k], r + tb.row_lo);
+  // untouched row (or an all-zero gradient): nothing changes.  Tested on g itself, not on its sum of squares: a row
+  // with |g| below ~1e-23 has sq == 0 in fp32 and still takes its step, as in the list kernels.
+  bool nz = false;
+#pragma unroll
+  for (int v = 0; v < NV; ++v)
+    if (lane * 4 + v * 128 < D) nz = nz || g[v].x != 0.f || g[v].y != 0.f || g[v].z != 0.f || g[v].w != 0.f;
+  const bool touched = __any_sync(0xffffffffu, nz);
   if (P.optimizer == DLRM_OPT_RWSADAGRAD) {
+    if (!touched) return;
     float sq = 0.f;
 #pragma unroll
     for (int v = 0; v < NV; ++v)
       if (lane * 4 + v * 128 < D)
         sq = fmaf(g[v].x, g[v].x, fmaf(g[v].y, g[v].y, fmaf(g[v].z, g[v].z, fmaf(g[v].w, g[v].w, sq))));
     sq = warp_sum(sq);
-    if (sq == 0.f) return;                  // untouched row (or an all-zero gradient): nothing changes
     const float m_new = tb.mom[(long long)r * tb.mom_stride] + sq * (1.0f / (float)D);
     const float stdv = sqrtf(m_new) + P.eps;
 #pragma unroll
@@ -182,11 +189,7 @@ __global__ void __launch_bounds__(256) emb_small_apply_kernel(const __grid_const
     if (lane == 0) tb.mom[(long long)r * tb.mom_stride] = m_new;
   } else {
     if constexpr (is_f16<wt>::value) {      // untouched rows are not rewritten
-      bool nz = false;
-#pragma unroll
-      for (int v = 0; v < NV; ++v)
-        if (lane * 4 + v * 128 < D) nz = nz || g[v].x != 0.f || g[v].y != 0.f || g[v].z != 0.f || g[v].w != 0.f;
-      if (!__any_sync(0xffffffffu, nz)) return;
+      if (!touched) return;
     }
 #pragma unroll
     for (int v = 0; v < NV; ++v)

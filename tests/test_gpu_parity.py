@@ -32,7 +32,7 @@ def _dev_batch(g: Golden, s):
 
 
 # ----------------------------------------------------------------------------- gather kernel
-@pytest.mark.parametrize("D", [2, 4, 8, 16, 32, 64, 100, 128, 256, 384])
+@pytest.mark.parametrize("D", [2, 4, 8, 12, 16, 32, 48, 64, 100, 128, 132, 256, 260, 384, 512, 516, 1000])
 @pytest.mark.parametrize("itype", [np.int64, np.int32])
 def test_emb_bag_fwd_bitexact(D, itype):
     from dlrm_b200 import _lib
