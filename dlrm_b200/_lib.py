@@ -11,7 +11,7 @@ from . import _build
 MAX_TABLES = 64
 ACT_NONE, ACT_RELU, ACT_SIGMOID = 0, 1, 2
 LOSS_MSE, LOSS_BCE, LOSS_WBCE = 0, 1, 2
-OPT_SGD, OPT_RWSADAGRAD = 0, 1
+OPT_SGD, OPT_RWSADAGRAD, OPT_ADAGRAD = 0, 1, 2
 GEMM_SIMT_FP32, GEMM_TC_BF16X3, GEMM_TC_BF16 = 0, 1, 2
 DTYPE_F32, DTYPE_F16 = 0, 1
 TUNE = dict(emb_bags_per_group=0, emb_unroll=1, emb_block=2, upd_block=3, gemm_splitk=4, gemm_smem_kb=5,

@@ -230,12 +230,14 @@ def run(argv=None):
                     emb_dtype=torch.float16 if args.emb_dtype == "fp16" else torch.float32)
     optimizer = lr_scheduler = None
     if not args.inference_only:
-        if args.optimizer == "sgd":
-            optimizer = fused.SGD(dlrm.parameters(), lr=args.learning_rate)
-        elif args.optimizer == "rwsadagrad":
-            optimizer = fused.RWSAdagrad(dlrm.parameters(), lr=args.learning_rate)
-        else:
-            sys.exit("ERROR: --optimizer=" + args.optimizer + " is not supported (sgd | rwsadagrad)")
+        opts = {"sgd": fused.SGD, "rwsadagrad": fused.RWSAdagrad, "adagrad": fused.Adagrad}   # :1342-1346
+        if args.optimizer not in opts:
+            sys.exit("ERROR: --optimizer=" + args.optimizer + " is not supported (sgd | rwsadagrad | adagrad)")
+        try:
+            optimizer = opts[args.optimizer](dlrm.parameters(), lr=args.learning_rate)
+        except fused.NotEngineParameters as e:
+            # the fused optimizers step the engine's memory: a model that is not a dlrm_b200.DLRM_Net cannot use them
+            sys.exit("ERROR: --optimizer=" + args.optimizer + " is not supported for this model (" + str(e) + ")")
         lr_scheduler = LRPolicy(optimizer, args.lr_num_warmup_steps, args.lr_decay_start_step,
                                 args.lr_num_decay_steps)
     if args.debug_mode:                                     # dlrm_s_pytorch.py:1222-1262, :1308-1311

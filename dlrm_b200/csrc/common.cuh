@@ -162,6 +162,18 @@ __device__ __forceinline__ unsigned filter_slot(const int* head_of_row, int log2
   return (unsigned)((key * 11400714819323198485ull) >> (64 - log2_size));
 }
 
+// Element-wise Adagrad (DLRM_OPT_ADAGRAD) on one element, in the order include/dlrm_b200.h states: the accumulator
+// takes g*g and the add as two roundings (torch's grad.pow(2) then the sparse add; no FMA contraction), then IEEE
+// sqrt, + eps, an IEEE division and one fused update w + nlr * q.  nlr = -lr.  Returns w'; s is updated in place.
+__device__ __forceinline__ float adagrad_ew(float g, float& s, float w, float nlr, float eps) {
+  s = __fadd_rn(s, __fmul_rn(g, g));
+  return fmaf(nlr, __fdiv_rn(g, __fadd_rn(__fsqrt_rn(s), eps)), w);
+}
+__device__ __forceinline__ float4 adagrad_ew4(float4 g, float4& s, float4 w, float nlr, float eps) {
+  return make_float4(adagrad_ew(g.x, s.x, w.x, nlr, eps), adagrad_ew(g.y, s.y, w.y, nlr, eps),
+                     adagrad_ew(g.z, s.z, w.z, nlr, eps), adagrad_ew(g.w, s.w, w.w, nlr, eps));
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -30,6 +30,11 @@
 //   fp16 tables (template row type wt = __half): the owner widens the row to fp32, applies the same fp32 step and
 //            stores the row with stochastic rounding (st_row4, common.cuh); the accumulator and the head stay
 //            fp32 / int32 words behind the row.  The float instantiations are the fp32 kernels.
+//   element-wise Adagrad (DLRM_OPT_ADAGRAD, template flag EW): the same coalesce and ownership; the owner also loads
+//            its row of per-element accumulators (momentum + r * mom_stride, a separate arena: 512 more bytes per row
+//            at D = 128, one more random access in and one out) in the same batch as the weight row, applies
+//            adagrad_ew (common.cuh: s += g*g with two roundings, IEEE sqrt, + eps, IEEE division, one fmaf) per
+//            element and stores both rows.  The EW = false instantiations are the SGD / RWSAdagrad kernels unchanged.
 #include "common.cuh"
 
 namespace dlrm {
@@ -381,8 +386,10 @@ __device__ __noinline__ void dup_sum_long(const EmbBwdParams& P, int nxt, int se
     for (int e = 0; e < W; ++e) g[v].x[e] = acc[v * W + e];
 }
 
-template <typename wt, int W, int NV, typename idx_t>
-__global__ void __launch_bounds__(256, NV == 1 ? 3 : 1) emb_update_kernel(const __grid_constant__ EmbBwdParams P,
+// EW: the element-wise Adagrad instantiation (DLRM_OPT_ADAGRAD): every lane also moves its columns of the row's
+// accumulator row, loaded with the weight row and stored with it.  EW = false is the SGD / RWSAdagrad kernel.
+template <typename wt, int W, int NV, typename idx_t, bool EW = false>
+__global__ void __launch_bounds__(256, NV == 1 ? (EW ? 2 : 3) : 1) emb_update_kernel(const __grid_constant__ EmbBwdParams P,
                                                                           int num_tables, long long total_hint) {
   __shared__ long long bound[DLRM_B200_MAX_TABLES_PER_CALL + 1], tend[DLRM_B200_MAX_TABLES_PER_CALL + 1];
   load_bounds<idx_t>(bound, tend, P, num_tables, total_hint);
@@ -395,7 +402,8 @@ __global__ void __launch_bounds__(256, NV == 1 ? 3 : 1) emb_update_kernel(const 
 #pragma unroll
   for (int v = 0; v < NV; ++v) col_ok[v] = lane * W + v * 32 * W < D;
   const float inv_d = 1.0f / (float)D;
-  constexpr int PF = NV == 1 ? 4 : 1;
+  // EW carries the accumulators too: 2 rows in flight at 2 CTAs per SM keep it free of spills (4 at 3 spill)
+  constexpr int PF = NV == 1 ? (EW ? 2 : 4) : 1;
 
   for (long long base = first + warp0 * 32; base < total; base += wstride * 32) {
     const long long pos = base + lane;
@@ -424,6 +432,7 @@ __global__ void __launch_bounds__(256, NV == 1 ? 3 : 1) emb_update_kernel(const 
     for (int u0 = 0; u0 < 32; u0 += PF) {
       if (((owners >> u0) & ((1u << PF) - 1u)) == 0u) continue;
       Pack<W> wpf[PF][NV], gpf[PF][NV];
+      Pack<W> spf[EW ? PF : 1][EW ? NV : 1];     // EW: the accumulators of the lane's columns
       float mpf[PF];
 #pragma unroll
       for (int u = 0; u < PF; ++u) {
@@ -441,7 +450,15 @@ __global__ void __launch_bounds__(256, NV == 1 ? 3 : 1) emb_update_kernel(const 
               wpf[u][v] = ld_pack<W>(wrow + lane * W + v * 32 * W);
               gpf[u][v] = ld_pack<W>(grow + lane * W + v * 32 * W);
             }
-          mpf[u] = (P.optimizer == DLRM_OPT_RWSADAGRAD) ? tb.mom[r * tb.mom_stride] : 0.f;
+          if constexpr (EW) {
+            const float* srow = tb.mom + r * tb.mom_stride;
+#pragma unroll
+            for (int v = 0; v < NV; ++v)
+              if (col_ok[v]) spf[u][v] = ld_pack<W>(srow + lane * W + v * 32 * W);
+            mpf[u] = 0.f;
+          } else {
+            mpf[u] = (P.optimizer == DLRM_OPT_RWSADAGRAD) ? tb.mom[r * tb.mom_stride] : 0.f;
+          }
         }
       }
 #pragma unroll
@@ -497,7 +514,20 @@ __global__ void __launch_bounds__(256, NV == 1 ? 3 : 1) emb_update_kernel(const 
             dup_sum_long<NV, W>(P, nxt0, self_bag, dyk_off, col_ok, g);
           }
         }
-        if (P.optimizer == DLRM_OPT_RWSADAGRAD) {
+        if constexpr (EW) {
+          (void)m_old;
+          const float nlr = -P.lr;
+          float* srow = tb.mom + r * tb.mom_stride;
+#pragma unroll
+          for (int v = 0; v < NV; ++v)
+            if (col_ok[v]) {
+              Pack<W> s = spf[u][v];
+#pragma unroll
+              for (int e = 0; e < W; ++e) w[v].x[e] = adagrad_ew(g[v].x[e], s.x[e], w[v].x[e], nlr, P.eps);
+              st_pack<W>(wrow + lane * W + v * 32 * W, w[v], is_f16<wt>::value ? sr_bits(rkey, lane + 32 * v) : 0ull);
+              st_pack<W>(srow + lane * W + v * 32 * W, s);
+            }
+        } else if (P.optimizer == DLRM_OPT_RWSADAGRAD) {
           float sq = 0.f;
 #pragma unroll
           for (int v = 0; v < NV; ++v)
@@ -609,7 +639,10 @@ __device__ __noinline__ float4 upd_sum_duplicates(const EmbBwdParams& P, int nxt
   return g;
 }
 
-template <typename wt, typename idx_t, int PF, int MINB>      // PF: row PAIRS in flight per warp
+// PF: row PAIRS in flight per warp.  EW: element-wise Adagrad (DLRM_OPT_ADAGRAD): every lane also loads its 8
+// accumulators (two float4 behind the row's accumulator pointer) in the same batch as the rows and stores them with
+// the row.  EW = false is the SGD / RWSAdagrad kernel.
+template <typename wt, typename idx_t, int PF, int MINB, bool EW = false>
 __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid_constant__ EmbBwdParams P, int num_tables,
                                                                     long long total_hint) {
   __shared__ long long bound[DLRM_B200_MAX_TABLES_PER_CALL + 1], tend[DLRM_B200_MAX_TABLES_PER_CALL + 1];
@@ -635,7 +668,7 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
   const long long wstep = (long long)gridDim.x * (blockDim.x >> 5) * 32;
   const float inv_d = 1.0f / (float)D;
   const float nlr = -P.lr;
-  const bool adagrad = P.optimizer == DLRM_OPT_RWSADAGRAD;
+  const bool adagrad = !EW && P.optimizer == DLRM_OPT_RWSADAGRAD;    // row-wise
   const int dbg = P.debug;
 
   for (long long base = first + warp0 * 32; base < total; base += wstep) {
@@ -663,7 +696,7 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
     const unsigned long long rkey =
         (is_f16<wt>::value && owner) ? sr_row_key(P.round_key[k], (long long)r + tb.row_lo) : 0ull;
     const float* gptr = owner ? dy_row(P, bag) + tb.dy_off : nullptr;
-    float* mptr = (owner && adagrad) ? tb.mom + (long long)r * tb.mom_stride : nullptr;
+    float* mptr = (owner && (adagrad || EW)) ? tb.mom + (long long)r * tb.mom_stride : nullptr;
     int* hptr = owner ? tb.head + (long long)r * tb.hs : nullptr;
     unsigned simple = __ballot_sync(0xffffffffu, owner && nxt == 0);
     unsigned dups = __ballot_sync(0xffffffffu, owner && nxt != 0);
@@ -671,6 +704,7 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
     // ---------------------------------------------------------------- rows without duplicates, two per step
     while (simple) {
       float4 wv[PF][2], gv[PF][2];
+      float4 sv[EW ? PF : 1][2];                   // EW: the lane's 8 accumulators
       float mv[PF];
       int sa[PF], sb[PF];
 #pragma unroll
@@ -701,6 +735,11 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
         gv[u][1] = (s_ >= 0 && c1_ok && ldg) ? *reinterpret_cast<const float4*>(gp + 4) : z;
         // the owning lanes load their accumulators in the same batch as the rows
         mv[u] = (adagrad && (lane == sa[u] || lane == sb[u])) ? *mptr : 0.f;
+        if constexpr (EW) {
+          const float* sp = reinterpret_cast<const float*>(__shfl_sync(0xffffffffu, (unsigned long long)mptr, sc)) + l16 * 8;
+          sv[u][0] = (s_ >= 0 && c0_ok) ? *reinterpret_cast<const float4*>(sp) : z;
+          sv[u][1] = (s_ >= 0 && c1_ok) ? *reinterpret_cast<const float4*>(sp + 4) : z;
+        }
       }
 #pragma unroll
       for (int u = 0; u < PF; ++u) {
@@ -721,12 +760,27 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
           if (lane == sb[u] && !(dbg & 4)) *mptr = mB;
         }
         wt* wp = reinterpret_cast<wt*>(__shfl_sync(0xffffffffu, (unsigned long long)wptr, sc)) + l16 * 8;
+        float* spw = nullptr;
+        float4 s0, s1;
+        if constexpr (EW) {                  // element-wise step: the accumulators move with the row
+          spw = reinterpret_cast<float*>(__shfl_sync(0xffffffffu, (unsigned long long)mptr, sc)) + l16 * 8;
+          s0 = sv[u][0]; s1 = sv[u][1];
+        }
         if constexpr (is_f16<wt>::value) {
           const unsigned long long rk = __shfl_sync(0xffffffffu, rkey, sc);
           if (s_ >= 0) {
             float4 w0 = wv[u][0], w1 = wv[u][1];
-            w0.x = fmaf(scale, g0.x, w0.x); w0.y = fmaf(scale, g0.y, w0.y); w0.z = fmaf(scale, g0.z, w0.z); w0.w = fmaf(scale, g0.w, w0.w);
-            w1.x = fmaf(scale, g1.x, w1.x); w1.y = fmaf(scale, g1.y, w1.y); w1.z = fmaf(scale, g1.z, w1.z); w1.w = fmaf(scale, g1.w, w1.w);
+            if constexpr (EW) {
+              w0 = adagrad_ew4(g0, s0, w0, nlr, P.eps);
+              w1 = adagrad_ew4(g1, s1, w1, nlr, P.eps);
+              if (c0_ok && !(dbg & 4)) {
+                *reinterpret_cast<float4*>(spw) = s0;
+                *reinterpret_cast<float4*>(spw + 4) = s1;
+              }
+            } else {
+              w0.x = fmaf(scale, g0.x, w0.x); w0.y = fmaf(scale, g0.y, w0.y); w0.z = fmaf(scale, g0.z, w0.z); w0.w = fmaf(scale, g0.w, w0.w);
+              w1.x = fmaf(scale, g1.x, w1.x); w1.y = fmaf(scale, g1.y, w1.y); w1.z = fmaf(scale, g1.z, w1.z); w1.w = fmaf(scale, g1.w, w1.w);
+            }
             if (c0_ok && !(dbg & 1)) {
               uint2 a, b;
               st_row4(reinterpret_cast<__half*>(&a), w0, sr_bits(rk, l16 * 2));
@@ -736,8 +790,15 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
           }
         } else if (s_ >= 0) {
           float4 w0 = wv[u][0], w1 = wv[u][1];
-          w0.x = fmaf(scale, g0.x, w0.x); w0.y = fmaf(scale, g0.y, w0.y); w0.z = fmaf(scale, g0.z, w0.z); w0.w = fmaf(scale, g0.w, w0.w);
-          w1.x = fmaf(scale, g1.x, w1.x); w1.y = fmaf(scale, g1.y, w1.y); w1.z = fmaf(scale, g1.z, w1.z); w1.w = fmaf(scale, g1.w, w1.w);
+          if constexpr (EW) {
+            w0 = adagrad_ew4(g0, s0, w0, nlr, P.eps);
+            w1 = adagrad_ew4(g1, s1, w1, nlr, P.eps);
+            if (c0_ok && !(dbg & 4)) *reinterpret_cast<float4*>(spw) = s0;
+            if (c1_ok && !(dbg & 4)) *reinterpret_cast<float4*>(spw + 4) = s1;
+          } else {
+            w0.x = fmaf(scale, g0.x, w0.x); w0.y = fmaf(scale, g0.y, w0.y); w0.z = fmaf(scale, g0.z, w0.z); w0.w = fmaf(scale, g0.w, w0.w);
+            w1.x = fmaf(scale, g1.x, w1.x); w1.y = fmaf(scale, g1.y, w1.y); w1.z = fmaf(scale, g1.z, w1.z); w1.w = fmaf(scale, g1.w, w1.w);
+          }
           if (c0_ok && !(dbg & 1)) *reinterpret_cast<float4*>(wp) = w0;
           if (c1_ok && !(dbg & 1)) *reinterpret_cast<float4*>(wp + 4) = w1;
         }
@@ -755,17 +816,28 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
       wt* wp = reinterpret_cast<wt*>(__shfl_sync(0xffffffffu, (unsigned long long)wptr, s_));
       float4 w = col_ok ? ld_row4(wp + lane * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
       const float m_old = (adagrad && lane == s_) ? *mptr : 0.f;
-      const float4 g = upd_sum_duplicates(P, nx, (int)(base + s_), sbg, dyo, lane, col_ok);
-      float scale = nlr;
-      if (adagrad) {
-        float sq = fmaf(g.x, g.x, fmaf(g.y, g.y, fmaf(g.z, g.z, g.w * g.w)));
-        sq = warp_sum(sq);
-        const float m_new = __shfl_sync(0xffffffffu, m_old, s_) + sq * inv_d;
-        scale = nlr / (sqrtf(m_new) + P.eps);
-        if (lane == s_) *mptr = m_new;
+      float* spd = nullptr;
+      float4 sd = make_float4(0.f, 0.f, 0.f, 0.f);
+      if constexpr (EW) {
+        spd = reinterpret_cast<float*>(__shfl_sync(0xffffffffu, (unsigned long long)mptr, s_)) + lane * 4;
+        if (col_ok) sd = *reinterpret_cast<const float4*>(spd);
       }
-      w.x = fmaf(scale, g.x, w.x); w.y = fmaf(scale, g.y, w.y);
-      w.z = fmaf(scale, g.z, w.z); w.w = fmaf(scale, g.w, w.w);
+      const float4 g = upd_sum_duplicates(P, nx, (int)(base + s_), sbg, dyo, lane, col_ok);
+      if constexpr (EW) {
+        w = adagrad_ew4(g, sd, w, nlr, P.eps);
+        if (col_ok) *reinterpret_cast<float4*>(spd) = sd;
+      } else {
+        float scale = nlr;
+        if (adagrad) {
+          float sq = fmaf(g.x, g.x, fmaf(g.y, g.y, fmaf(g.z, g.z, g.w * g.w)));
+          sq = warp_sum(sq);
+          const float m_new = __shfl_sync(0xffffffffu, m_old, s_) + sq * inv_d;
+          scale = nlr / (sqrtf(m_new) + P.eps);
+          if (lane == s_) *mptr = m_new;
+        }
+        w.x = fmaf(scale, g.x, w.x); w.y = fmaf(scale, g.y, w.y);
+        w.z = fmaf(scale, g.z, w.z); w.w = fmaf(scale, g.w, w.w);
+      }
       if constexpr (is_f16<wt>::value) {
         const unsigned long long rk = __shfl_sync(0xffffffffu, rkey, s_);
         if (col_ok) st_row4(wp + lane * 4, w, sr_bits(rk, lane));
@@ -840,6 +912,9 @@ extern "C" int dlrm_b200_emb_bwd_link(const dlrm_emb_bwd_table_t* tables, int nu
   return 0;
 }
 
+// Lean-kernel shape of the element-wise Adagrad instantiation: row pairs in flight per warp, CTAs per SM.
+constexpr int EW_PF = 2, EW_MINB = 2;
+
 static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, int dim, int64_t batch,
                            int idx_bytes, int include_last, const int32_t* next, const float* dY,
                            int64_t dy_stride_sample, int64_t dy_stride_table, int optimizer, float lr,
@@ -849,8 +924,9 @@ static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, i
   EmbBwdParams P{};
   if (int rc = fill_params(P, tables, num_tables, "emb_bwd_update")) return rc;
   if (idx_bytes != 4 && idx_bytes != 8) return set_error("emb_bwd_update: idx_bytes=%d", idx_bytes);
-  if (optimizer != DLRM_OPT_SGD && optimizer != DLRM_OPT_RWSADAGRAD)
+  if (optimizer != DLRM_OPT_SGD && optimizer != DLRM_OPT_RWSADAGRAD && optimizer != DLRM_OPT_ADAGRAD)
     return set_error("emb_bwd_update: optimizer=%d", optimizer);
+  const bool ew = optimizer == DLRM_OPT_ADAGRAD;
   if (dim <= 0 || dim > 1024) return set_error("emb_bwd_update: dim=%d unsupported (1..1024)", dim);
   const bool f16 = num_tables > 0 && tables[0].weight_dtype == DLRM_DTYPE_F16;
   if (f16 && dim % 8) return set_error("emb_bwd_update: fp16 tables need dim %% 8 == 0 (dim=%d)", dim);
@@ -877,8 +953,13 @@ static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, i
     P.t[k].dy_off = tables[k].use_dy_off ? tables[k].dy_off : (int64_t)k * dy_stride_table;
     vec = vec && (P.t[k].dy_off % 4 == 0);
     if (!tables[k].weight) return set_error("emb_bwd_update: table %d weight NULL", k);
-    if (optimizer == DLRM_OPT_RWSADAGRAD && !tables[k].momentum)
+    if ((optimizer == DLRM_OPT_RWSADAGRAD || ew) && !tables[k].momentum)
       return set_error("emb_bwd_update: table %d momentum NULL", k);
+    if (ew) {     // one accumulator per element: rows of at least dim floats, the vector kernels need 16-byte ones
+      P.t[k].mom_stride = tables[k].mom_stride > 0 ? tables[k].mom_stride : dim;
+      if (P.t[k].mom_stride < dim) return set_error("emb_bwd_update: table %d: Adagrad mom_stride < dim", k);
+      vec = vec && aligned16(tables[k].momentum) && P.t[k].mom_stride % 4 == 0;
+    }
     vec = vec && aligned16(tables[k].weight);
     if (P.t[k].ld <= 0) P.t[k].ld = dim;
     if (P.t[k].ld < dim) return set_error("emb_bwd_update: table %d: ld < dim", k);
@@ -914,19 +995,29 @@ static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, i
   if (gridx < 1) gridx = 1;
   const long long total_hint = include_last ? 0 : (tables[num_tables - 1].pair_base + tables[num_tables - 1].nnz);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-#define UPD_T(WT, Wd, NV)                                                                                  \
-  do {                                                                                                     \
-    if (idx_bytes == 8)                                                                                    \
-      emb_update_kernel<WT, Wd, NV, long long><<<(unsigned)gridx, block, 0, st>>>(P, num_tables, total_hint); \
-    else                                                                                                   \
-      emb_update_kernel<WT, Wd, NV, int><<<(unsigned)gridx, block, 0, st>>>(P, num_tables, total_hint);    \
-    DLRM_CHECK_LAUNCH("emb_update_kernel");                                                                \
-    return 0;                                                                                              \
+#define UPD_E(WT, Wd, NV, EW)                                                                                \
+  do {                                                                                                           \
+    if (idx_bytes == 8)                                                                                          \
+      emb_update_kernel<WT, Wd, NV, long long, EW><<<(unsigned)gridx, block, 0, st>>>(P, num_tables, total_hint); \
+    else                                                                                                         \
+      emb_update_kernel<WT, Wd, NV, int, EW><<<(unsigned)gridx, block, 0, st>>>(P, num_tables, total_hint);      \
+    DLRM_CHECK_LAUNCH("emb_update_kernel");                                                                      \
+    return 0;                                                                                                    \
+  } while (0)
+#define UPD_T(WT, Wd, NV)   \
+  do {                      \
+    if (ew) UPD_E(WT, Wd, NV, true); \
+    UPD_E(WT, Wd, NV, false);        \
   } while (0)
 #define UPD(Wd, NV) UPD_T(float, Wd, NV)
+#define LEAN(WT, IDX)                                                                                              \
+  do {                                                                                                             \
+    if (ew) emb_update_lean_kernel<WT, IDX, EW_PF, EW_MINB, true><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint); \
+    else emb_update_lean_kernel<WT, IDX, 2, 3><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);        \
+  } while (0)
   if (f16 && !vec)
     return set_error("emb_bwd_update: fp16 tables need a 16-byte aligned weight pointer, ld %% 4 == 0 (8-byte rows) "
-                     "and 16-byte aligned gradient rows");
+                     "and 16-byte aligned gradient rows%s", ew ? " and accumulators (momentum, mom_stride % 4 == 0)" : "");
   if (vec && lean_rows && dim <= 128 && !P.flags && get_tunable(TUNE_UPD_LEAN) != 2) {
     long long gl = (total / 32 + block / 32) / (block / 32);
     if (gl > (long long)sms * 3) gl = (long long)sms * 3;
@@ -934,13 +1025,14 @@ static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, i
     // 3 CTAs of 256 threads per SM (<= 85 registers), 2 row pairs in flight per warp: on H100 (cfg3) 3 pairs /
     // 3 CTAs and 4 pairs / 2 CTAs per SM were measured no faster and 8 % slower.  The kernel is bound by the RATE of random accesses
     // (row + accumulator read, row + accumulator + head write), not by the latency of any one of them.
+    // Element-wise Adagrad carries 16 more floats per row pair (the accumulators): EW_PF / EW_MINB above.
     if (f16) {
-      if (idx_bytes == 8) emb_update_lean_kernel<__half, long long, 2, 3><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);
-      else emb_update_lean_kernel<__half, int, 2, 3><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);
+      if (idx_bytes == 8) LEAN(__half, long long);
+      else LEAN(__half, int);
     } else if (idx_bytes == 8) {
-      emb_update_lean_kernel<float, long long, 2, 3><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);
+      LEAN(float, long long);
     } else {
-      emb_update_lean_kernel<float, int, 2, 3><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);
+      LEAN(float, int);
     }
     DLRM_CHECK_LAUNCH("emb_update_lean_kernel");
     return 0;
@@ -963,8 +1055,10 @@ static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, i
   if (dim <= 256) UPD(1, 8);
   if (dim <= 512) UPD(1, 16);
   UPD(1, 32);
+#undef LEAN
 #undef UPD
 #undef UPD_T
+#undef UPD_E
 }
 
 extern "C" int dlrm_b200_emb_bwd_update(const dlrm_emb_bwd_table_t* tables, int num_tables, int dim,

@@ -135,7 +135,8 @@ __global__ void __launch_bounds__(256) emb_small_accum_kernel(const __grid_const
     *reinterpret_cast<float4*>(dst + e) = *reinterpret_cast<const float4*>(acc + e);
 }
 
-template <typename wt, int NV>
+// EW: element-wise Adagrad (DLRM_OPT_ADAGRAD): the lane's columns of the row's accumulator row move with the row.
+template <typename wt, int NV, bool EW = false>
 __global__ void __launch_bounds__(256) emb_small_apply_kernel(const __grid_constant__ SmallParams P, int num_tables) {
   const int lane = threadIdx.x & 31;
   const int grow = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);   // row in the partial row space
@@ -168,7 +169,20 @@ __global__ void __launch_bounds__(256) emb_small_apply_kernel(const __grid_const
   for (int v = 0; v < NV; ++v)
     if (lane * 4 + v * 128 < D) nz = nz || g[v].x != 0.f || g[v].y != 0.f || g[v].z != 0.f || g[v].w != 0.f;
   const bool touched = __any_sync(0xffffffffu, nz);
-  if (P.optimizer == DLRM_OPT_RWSADAGRAD) {
+  if constexpr (EW) {
+    // a row whose gradient is all zero changes neither w nor s (torch: s + 0, w + 0): not stepped, not rewritten
+    if (!touched) return;
+    float* srow = tb.mom + (long long)r * tb.mom_stride + lane * 4;
+#pragma unroll
+    for (int v = 0; v < NV; ++v)
+      if (lane * 4 + v * 128 < D) {
+        float4 w = ld_row4(wrow + v * 128);
+        float4 sv = *reinterpret_cast<const float4*>(srow + v * 128);
+        w = adagrad_ew4(g[v], sv, w, nlr, P.eps);
+        st_row4(wrow + v * 128, w, is_f16<wt>::value ? sr_bits(rkey, lane + 32 * v) : 0ull);
+        *reinterpret_cast<float4*>(srow + v * 128) = sv;
+      }
+  } else if (P.optimizer == DLRM_OPT_RWSADAGRAD) {
     if (!touched) return;
     float sq = 0.f;
 #pragma unroll
@@ -218,7 +232,9 @@ extern "C" int dlrm_b200_emb_bwd_small_update(const dlrm_emb_bwd_table_t* tables
   if (num_tables == 0 || batch == 0) return 0;
   if (num_tables < 0 || num_tables > SMALL_MAX_TABLES) return set_error("emb_bwd_small_update: num_tables=%d (max %d)", num_tables, SMALL_MAX_TABLES);
   if (idx_bytes != 4 && idx_bytes != 8) return set_error("emb_bwd_small_update: idx_bytes=%d", idx_bytes);
-  if (optimizer != DLRM_OPT_SGD && optimizer != DLRM_OPT_RWSADAGRAD) return set_error("emb_bwd_small_update: optimizer=%d", optimizer);
+  if (optimizer != DLRM_OPT_SGD && optimizer != DLRM_OPT_RWSADAGRAD && optimizer != DLRM_OPT_ADAGRAD)
+    return set_error("emb_bwd_small_update: optimizer=%d", optimizer);
+  const bool ew = optimizer == DLRM_OPT_ADAGRAD;
   if (dim <= 0 || dim % 4 || dim > 512) return set_error("emb_bwd_small_update: dim=%d (multiple of 4, <= 512)", dim);
   if (!tables || !scratch || (!dY && !peer_dY)) return set_error("emb_bwd_small_update: NULL pointer");
   if (dy_stride_sample % 4) return set_error("emb_bwd_small_update: dY rows must be 16-byte aligned");
@@ -232,7 +248,7 @@ extern "C" int dlrm_b200_emb_bwd_small_update(const dlrm_emb_bwd_table_t* tables
     if (s.weight_dtype != dtype)
       return set_error("emb_bwd_small_update: table %d: weight_dtype differs from table 0's (one row type per call)", k);
     if (!s.weight || !s.offsets || (!s.indices && s.nnz > 0)) return set_error("emb_bwd_small_update: table %d NULL pointer", k);
-    if (optimizer == DLRM_OPT_RWSADAGRAD && !s.momentum) return set_error("emb_bwd_small_update: table %d momentum NULL", k);
+    if ((optimizer == DLRM_OPT_RWSADAGRAD || ew) && !s.momentum) return set_error("emb_bwd_small_update: table %d momentum NULL", k);
     const int64_t rn = s.row_n > 0 ? s.row_n : s.rows;
     if (rn <= 0 || rn > 4096) return set_error("emb_bwd_small_update: table %d has %lld rows (1..4096)", k, (long long)rn);
     if (!s.use_dy_off || s.dy_off % 4) return set_error("emb_bwd_small_update: table %d needs a 16-byte aligned dy_off", k);
@@ -242,6 +258,12 @@ extern "C" int dlrm_b200_emb_bwd_small_update(const dlrm_emb_bwd_table_t* tables
     t.dy_off = s.dy_off; t.row_lo = s.row_n > 0 ? s.row_lo : 0; t.row_n = (int)rn; t.part_row0 = total_rows;
     P.round_key[k] = s.round_key;
     if (t.ld % 4 || (reinterpret_cast<uintptr_t>(t.w) & 15)) return set_error("emb_bwd_small_update: table %d rows not 16-byte aligned", k);
+    if (ew) {     // one accumulator per element, in rows of at least dim floats on 16-byte boundaries
+      t.mom_stride = s.mom_stride > 0 ? s.mom_stride : dim;
+      if (t.mom_stride < dim) return set_error("emb_bwd_small_update: table %d: Adagrad mom_stride < dim", k);
+      if (t.mom_stride % 4 || (reinterpret_cast<uintptr_t>(t.mom) & 15))
+        return set_error("emb_bwd_small_update: table %d: Adagrad accumulators not 16-byte aligned", k);
+    }
     total_rows += (int)rn;
     max_rows = (int)rn > max_rows ? (int)rn : max_rows;
   }
@@ -271,10 +293,11 @@ extern "C" int dlrm_b200_emb_bwd_small_update(const dlrm_emb_bwd_table_t* tables
                                      200 * 1024));                                                                    \
     emb_small_accum_kernel<NV, IDX><<<dim3((unsigned)chunks, (unsigned)num_tables), 256, smem, st>>>(P);              \
     DLRM_CHECK_LAUNCH("emb_small_accum_kernel");                                                                      \
-    if (dtype == DLRM_DTYPE_F16)                                                                                      \
-      emb_small_apply_kernel<__half, NV><<<(unsigned)((total_rows + 7) / 8), 256, 0, st>>>(P, num_tables);            \
-    else                                                                                                              \
-      emb_small_apply_kernel<float, NV><<<(unsigned)((total_rows + 7) / 8), 256, 0, st>>>(P, num_tables);             \
+    const unsigned ga = (unsigned)((total_rows + 7) / 8);                                                             \
+    if (dtype == DLRM_DTYPE_F16 && ew) emb_small_apply_kernel<__half, NV, true><<<ga, 256, 0, st>>>(P, num_tables);   \
+    else if (dtype == DLRM_DTYPE_F16) emb_small_apply_kernel<__half, NV><<<ga, 256, 0, st>>>(P, num_tables);          \
+    else if (ew) emb_small_apply_kernel<float, NV, true><<<ga, 256, 0, st>>>(P, num_tables);                          \
+    else emb_small_apply_kernel<float, NV><<<ga, 256, 0, st>>>(P, num_tables);                                        \
     DLRM_CHECK_LAUNCH("emb_small_apply_kernel");                                                                      \
     return 0;                                                                                                         \
   } while (0)

@@ -117,6 +117,7 @@ extern "C" int dlrm_b200_dense_update(float* param, const float* grad, float* st
                                       int optimizer, float lr, float eps, void* stream) {
   using namespace dlrm;
   if (n == 0) return 0;
+  if (optimizer == DLRM_OPT_ADAGRAD) optimizer = DLRM_OPT_RWSADAGRAD;   // the dense branches are the same algorithm
   if (optimizer != DLRM_OPT_SGD && optimizer != DLRM_OPT_RWSADAGRAD)
     return set_error("dense_update: optimizer=%d", optimizer);
   if (!param || !grad || (optimizer == DLRM_OPT_RWSADAGRAD && !state))

@@ -104,6 +104,7 @@ extern "C" int dlrm_b200_dense_update_pack(const dlrm_dense_layer_t* layers, int
   using namespace dlrm;
   if (num_layers <= 0) return 0;
   if (num_layers > 16) return set_error("dense_update_pack: at most 16 layers per call (got %d)", num_layers);
+  if (optimizer == DLRM_OPT_ADAGRAD) optimizer = DLRM_OPT_RWSADAGRAD;   // the dense branches are the same algorithm
   if (optimizer < -2 || optimizer > DLRM_OPT_RWSADAGRAD) return set_error("dense_update_pack: optimizer=%d", optimizer);
   DenseLayers P;
   long long ctas = 0;

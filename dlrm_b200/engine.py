@@ -14,6 +14,8 @@ HBM layout (fp32 unless noted)
   tables   [sum_k rows_k, D]   one allocation; table k = rows [row_base_k, row_base_k + rows_k)
                                (emb_dtype="fp16": fp16 rows [D halves | fp32 accumulator | int32 head | pad])
   momentum [sum_k rows_k]      RWSAdagrad row-wise accumulator (optim/rwsadagrad.py:91-95)
+  acc_ew   [sum_k rows_k, D]   element-wise Adagrad accumulator (torch.optim.Adagrad 'sum'), a separate arena
+                               allocated by the first Adagrad step; same row_base as the tables
   head     [sum_k rows_k] i32  per-row list heads for the sort-free coalesce (zero between steps)
   mark     [nnz] u8            per-occurrence superseded marks beside link[] (zero between steps)
   dense    [P]                 bot W0,b0,W1,b1,... top W0,b0,...  (+ grad arena, + Adagrad sums)
@@ -34,10 +36,11 @@ import torch
 
 from . import _lib
 from ._lib import (ACT_NONE, ACT_RELU, ACT_SIGMOID, DTYPE_F16, DTYPE_F32, GEMM_SIMT_FP32, LOSS_BCE, LOSS_MSE,
-                   LOSS_WBCE, OPT_RWSADAGRAD, OPT_SGD, EmbBwdTable, EmbFwdTable)
+                   LOSS_WBCE, OPT_ADAGRAD, OPT_RWSADAGRAD, OPT_SGD, EmbBwdTable, EmbFwdTable)
 
 _LOSS = {"mse": LOSS_MSE, "bce": LOSS_BCE, "wbce": LOSS_WBCE}
-_OPT = {"sgd": OPT_SGD, "rwsadagrad": OPT_RWSADAGRAD}
+_OPT = {"sgd": OPT_SGD, "rwsadagrad": OPT_RWSADAGRAD, "adagrad": OPT_ADAGRAD}
+_LR_DECAY = ("rwsadagrad", "adagrad")     # optimizers whose step applies lr_decay: clr = lr / (1 + (step - 1) lr_decay)
 
 
 def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
@@ -191,6 +194,7 @@ class Engine:
         self.tables = torch.zeros((self.total_rows, self.ldw), dtype=self.wdtype, device=dev)
         self._head_sep = None if self.interleave else torch.zeros(self.total_rows, dtype=torch.int32, device=dev)
         self._momentum_sep: Optional[torch.Tensor] = None
+        self.acc_ew: Optional[torch.Tensor] = None       # element-wise Adagrad accumulators [total_rows, D]
         self.row_weights: Optional[torch.Tensor] = None  # weighted pooling v_W_l, arena [total_rows]
         # ---- dense arena
         self.dense_slices = []  # (name, layer, kind, offset, shape)
@@ -406,8 +410,24 @@ class Engine:
         if optimizer == "rwsadagrad":
             if not self.interleave and self._momentum_sep is None:
                 self._momentum_sep = torch.zeros(self.total_rows, dtype=torch.float32, device=self.device)
-            if self.dense_state is None:
-                self.dense_state = torch.zeros_like(self.dense)
+        if optimizer == "adagrad" and self.acc_ew is None:
+            # One fp32 accumulator per table element (4 D bytes per row), in its own arena: the optimizer is created
+            # after the tables are laid out (dlrm_s_pytorch.py builds DLRM_Net first), and moving the tables into an
+            # interleaved [w | s] layout then would move every emb_l[k].weight.
+            self.acc_ew = torch.zeros((self.total_rows, self.D), dtype=torch.float32, device=self.device)
+        if optimizer in _LR_DECAY and self.dense_state is None:
+            self.dense_state = torch.zeros_like(self.dense)
+
+    def accumulator_ew(self, k: int) -> torch.Tensor:
+        """[rows_k, D] element-wise Adagrad accumulators of table k (after ensure_optimizer_state("adagrad"))."""
+        return self.acc_ew[int(self.row_base[k]):int(self.row_base[k + 1])]
+
+    def _point_at_acc_ew(self, desc, ks):
+        """Element-wise Adagrad: the descriptors of tables ks take the [rows, D] accumulator rows as `momentum`."""
+        base = self.acc_ew.data_ptr()
+        for n, k in enumerate(ks):
+            desc[n].momentum = base + int(self.row_base[k]) * self.D * 4
+            desc[n].mom_stride = self.D
 
     # ------------------------------------------------------------------ parameters
     def mark_params_changed(self):
@@ -738,6 +758,8 @@ class Engine:
             for c0 in range(0, len(small), 32):
                 ks = small[c0:c0 + 32]
                 desc, _ = self._bwd_desc_chunk(sp, ks, dy_off)
+                if optimizer == "adagrad":
+                    self._point_at_acc_ew(desc, ks)
                 rows = sum(self.ln_emb[k] for k in ks)
                 need = int(self.lib.dlrm_b200_emb_bwd_small_scratch_bytes(rows, self.D, sp.batch))
                 if getattr(self, "small_scratch", None) is None or self.small_scratch.numel() * 4 < need:
@@ -751,6 +773,8 @@ class Engine:
         for c0 in range(0, len(big), _lib.MAX_TABLES):
             ks = big[c0:c0 + _lib.MAX_TABLES]
             desc, _ = self._bwd_desc_chunk(sp, ks, dy_off)
+            if optimizer == "adagrad":
+                self._point_at_acc_ew(desc, ks)
             dd = C.byref(self.dedup) if self._filtered else None
             if peer is not None:
                 _lib.check(self.lib.dlrm_b200_emb_bwd_update_p2p(desc, len(ks), self.D, sp.batch, sp.idx_bytes,
@@ -939,7 +963,7 @@ class Engine:
         self._join_update = bool(join_update) or not self.tc or not self.multi_stream
         self.forward(X, sp, link=not link_done, skip_head=True)
         self.opt_step += 1
-        clr = lr / (1.0 + (self.opt_step - 1.0) * lr_decay) if optimizer == "rwsadagrad" else lr
+        clr = lr / (1.0 + (self.opt_step - 1.0) * lr_decay) if optimizer in _LR_DECAY else lr
         if self.tc:
             self.backward(X, sp, target, update=(optimizer, clr))
         else:

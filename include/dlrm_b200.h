@@ -44,8 +44,8 @@ extern "C" {
 enum { DLRM_ACT_NONE = 0, DLRM_ACT_RELU = 1, DLRM_ACT_SIGMOID = 2 };
 /* loss functions (dlrm_s_pytorch.py:385-393) */
 enum { DLRM_LOSS_MSE = 0, DLRM_LOSS_BCE = 1, DLRM_LOSS_WBCE = 2 };
-/* sparse optimizers: torch.optim.SGD (dlrm_s_pytorch.py:1343) / optim/rwsadagrad.py */
-enum { DLRM_OPT_SGD = 0, DLRM_OPT_RWSADAGRAD = 1 };
+/* sparse optimizers: torch.optim.SGD (dlrm_s_pytorch.py:1343) / optim/rwsadagrad.py / torch.optim.Adagrad (:1345) */
+enum { DLRM_OPT_SGD = 0, DLRM_OPT_RWSADAGRAD = 1, DLRM_OPT_ADAGRAD = 2 };
 /* GEMM back ends */
 enum { DLRM_GEMM_SIMT_FP32 = 0, DLRM_GEMM_TC_BF16X3 = 1, DLRM_GEMM_TC_BF16 = 2 };
 /* storage type of embedding table rows (weight_dtype of the table descriptors) */
@@ -114,7 +114,17 @@ int dlrm_b200_emb_bag_fwd(const dlrm_emb_fwd_table_t* tables /*[host]*/, int num
  * with an order-independent fixed-point sum (the same result on every run), then
  *   RWSAdagrad: momentum[row] += mean_d(g^2); W[row] -= lr * g / (sqrt(momentum[row]) + eps)
  *   SGD:        W[row] -= lr * g
- * `lr` is the already-decayed clr of optim/rwsadagrad.py:115.
+ *   Adagrad (element-wise, torch.optim.Adagrad on a sparse gradient): for every column j of the row,
+ *               s = momentum[row * mom_stride + j]
+ *               s = __fadd_rn(s, __fmul_rn(g[j], g[j]))       (two roundings, no FMA: grad.pow(2), then the add)
+ *               d = sqrtf(s) + eps                             (IEEE sqrt, then one rounding)
+ *               W[row][j] = fmaf(-lr, g[j] / d, W[row][j])     (IEEE division; one fused step)
+ *             `momentum` then points at a [rows][mom_stride] fp32 array (one accumulator per element; mom_stride 0
+ *             means dim, otherwise it must be >= dim); NULL momentum or 0 < mom_stride < dim is an error without a
+ *             launch.  The vector kernels need a 16-byte aligned momentum and mom_stride % 4 == 0; other
+ *             accumulators take the scalar kernel (fp16 tables and the tiny-table path have none: an error).
+ *             Rows that do not occur are not touched, neither their weights nor their accumulators.
+ * `lr` is the already-decayed clr of optim/rwsadagrad.py:115 (torch.optim.Adagrad: lr / (1 + (step - 1) lr_decay)).
  * fp16 tables (weight_dtype = DLRM_DTYPE_F16): the row is widened to fp32, the step above runs in fp32 with the
  * operations of the fp32 kernel, and the result x is stored with STOCHASTIC ROUNDING: x itself when it is an
  * fp16 value, else lo (the fp16 neighbour toward zero) or hi (the one away from zero), hi iff
@@ -126,7 +136,7 @@ int dlrm_b200_emb_bag_fwd(const dlrm_emb_fwd_table_t* tables /*[host]*/, int num
  * ------------------------------------------------------------------------------------------ */
 typedef struct {
   float* weight;        /* [rows, dim] updated in place */
-  float* momentum;      /* [rows] (RWSAdagrad) or NULL (SGD) */
+  float* momentum;      /* [rows] (RWSAdagrad), [rows][mom_stride] (Adagrad) or NULL (SGD) */
   int32_t* head;        /* [rows] zero-initialised scratch, self-cleaning */
   const void* indices;  /* as in forward */
   const void* offsets;
@@ -136,7 +146,7 @@ typedef struct {
   int64_t ld;           /* row stride of `weight` in elements of the row type; 0 = dim.  fp16: the weight pointer
                          * 16-byte aligned and ld % 4 == 0 (rows on 8-byte boundaries); ld % 8 == 0 (16-byte rows, the
                          * engine's layout) lets dim <= 128 take the faster kernel with one 16-byte access per lane */
-  int64_t mom_stride;   /* elements between consecutive rows' accumulators in `momentum`; 0 = 1.
+  int64_t mom_stride;   /* elements between consecutive rows' accumulators in `momentum`; 0 = 1 (Adagrad: 0 = dim).
                          * ld = dim + 4 with momentum = weight + dim and mom_stride = ld keeps the
                          * row-wise Adagrad accumulator in the SAME DRAM burst as its row: the update then
                          * costs one activation per row instead of two. */
@@ -328,6 +338,8 @@ int dlrm_b200_act_bwd(const float* gy, const float* y, float* gz, int64_t n, int
  * Dense parameters of optimizer.step(): flat arenas (all bot/top W and b, contiguous).
  *   SGD:        p -= lr * g
  *   RWSAdagrad dense branch (optim/rwsadagrad.py:145-148): s += g*g; p -= lr * g / (sqrt(s)+eps)
+ *   Adagrad: the same algorithm, so DLRM_OPT_ADAGRAD runs exactly what DLRM_OPT_RWSADAGRAD runs here and in
+ *   dlrm_b200_dense_update_pack.
  * ------------------------------------------------------------------------------------------ */
 /* ------------------------------------------------------------------------------------------
  * Fused head for a top MLP whose last layer has one output: Linear(K->1) + act + clamp + loss
