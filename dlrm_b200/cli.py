@@ -2,12 +2,15 @@
 the H100 engine, so that `bench/dlrm_s_benchmark.sh` runs unmodified from this repo's root.
 
 Every flag of the reference is accepted with the same default.  Flags that select subsystems outside
-the hot path (datasets, QR/MD embeddings, quantisation, ONNX, mlperf logging, ...) exit with the
-reference's style of error.  --test-freq / --inference-only run the reference's test pass (inference(),
+the hot path (datasets other than the MLPerf binary Terabyte records, QR/MD embeddings, quantisation,
+ONNX, ...) exit with the reference's style of error.  `--data-generation=dataset --mlperf-logging
+--memory-map --data-set=terabyte --mlperf-bin-loader` trains on the MLPerf binary records, decoded on
+the GPU (binrecords.DeviceBatches), and --mlperf-logging prints the reference's MLPerf metric line,
+computed on the GPU (metrics.py).  --test-freq / --inference-only run the reference's test pass (inference(),
 :759-900), --save-model / --load-model write and read the reference's checkpoint dictionary (:860-866,
 :1399-1456, :1703-1715; a checkpoint written by the reference loads here and vice versa), --enable-profiling
-and --debug-mode do what they do there.  --max-ind-range and --mlperf-grad-accum-iter only act on the
-dataset / mlperf-logging paths in the reference (rejected above), so they have no effect here either.  The random-data generator draws from numpy's global RNG in EXACTLY the
+and --debug-mode do what they do there.  --max-ind-range acts on the binary records only, as in
+the reference; --mlperf-grad-accum-iter other than 1 is rejected.  The random-data generator draws from numpy's global RNG in EXACTLY the
 reference's order (dlrm_data_pytorch.py:899-960 and :838-846; re-seeded at batch 0 of every epoch,
 :637-638), and parameters are initialised in the reference's order, so for the same
 `--numpy-rand-seed` the inputs and initial weights are bit-identical to the reference's and the printed
@@ -156,12 +159,26 @@ class LRPolicy:
 def run(argv=None):
     args = build_parser().parse_args(argv)
     for flag, name in ((args.qr_flag, "--qr-flag"), (args.md_flag, "--md-flag"), (args.save_onnx, "--save-onnx"),
-                       (args.mlperf_logging, "--mlperf-logging"), (args.plot_compute_graph, "--plot-compute-graph")):
+                       (args.plot_compute_graph, "--plot-compute-graph")):
         if flag:
             sys.exit("ERROR: %s is outside the dlrm_b200 hot path (SURVEY.md section 2)" % name)
-    if args.data_generation not in ("random", "synthetic"):
+    # the reference's condition for its MLPerf binary loader (dlrm_data_pytorch.py:415-419); other datasets stay out
+    bin_loader = (args.data_generation == "dataset" and args.mlperf_logging and args.memory_map
+                  and args.data_set == "terabyte" and args.mlperf_bin_loader)
+    if args.data_generation not in ("random", "synthetic") and not bin_loader:
         sys.exit("ERROR: --data-generation=" + args.data_generation + " is not supported (datasets are outside "
-                 "the dlrm_b200 hot path; use random or synthetic)")
+                 "the dlrm_b200 hot path; use random or synthetic, or the MLPerf binary loader: --mlperf-logging "
+                 "--memory-map --data-set=terabyte --mlperf-bin-loader)")
+    if args.mlperf_logging and args.mlperf_grad_accum_iter != 1:
+        sys.exit("ERROR: --mlperf-grad-accum-iter=%d is not supported (1)" % args.mlperf_grad_accum_iter)
+    if args.mlperf_logging and not bin_loader and not args.round_targets:
+        sys.exit("ERROR: --mlperf-logging computes classification metrics: random targets need --round-targets=True")
+    if bin_loader and int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        sys.exit("ERROR: --data-generation=dataset runs on one GPU (sharded runs need one global batch size; "
+                 "test and tail batches differ)")
+    if args.mlperf_logging and int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        sys.exit("ERROR: --mlperf-logging runs on one GPU (the device-side test metrics of a sharded run, which would "
+                 "need every rank's scores gathered, are not supported)")
     if args.quantize_emb_with_bit in [4, 8] or args.quantize_mlp_with_bit != 32:
         sys.exit("ERROR: 4 and 8-bit quantization on GPU is not supported")
     if not torch.cuda.is_available():
@@ -194,7 +211,26 @@ def run(argv=None):
     from .dlrm_net import DLRM_Net
 
     ln_bot = np.fromstring(args.arch_mlp_bot, dtype=int, sep="-")
-    ln_emb = np.fromstring(args.arch_embedding_size, dtype=int, sep="-")
+    if bin_loader:                                           # dlrm_s_pytorch.py:1104-1124, dlrm_data_pytorch.py:420-425
+        from . import binrecords
+
+        if args.test_mini_batch_size < 0:
+            args.test_mini_batch_size = args.mini_batch_size
+        lstr = args.processed_data_file.split("/")
+        d_path = "/".join(lstr[0:-1]) + "/" + lstr[-1].split(".")[0]
+        files = (d_path + "_train.bin", d_path + "_test.bin", args.raw_data_file + "_fea_count.npz")
+        for f in files:
+            if not os.path.exists(f):
+                sys.exit("ERROR: " + f + " does not exist (preprocessing raw Criteo days is not supported: "
+                         "make the MLPerf binary files with the reference's data_loader_terabyte.py)")
+        train_ds = binrecords.CriteoBinDataset(files[0], files[2], args.mini_batch_size, args.max_ind_range)
+        test_ds = binrecords.CriteoBinDataset(files[1], files[2], args.test_mini_batch_size, args.max_ind_range)
+        ln_emb = np.asarray(train_ds.counts)
+        if args.max_ind_range > 0:
+            ln_emb = np.minimum(ln_emb, args.max_ind_range)
+        ln_bot[0] = train_ds.m_den
+    else:
+        ln_emb = np.fromstring(args.arch_embedding_size, dtype=int, sep="-")
     m_den = ln_bot[0]
     m_spa = args.arch_sparse_feature_size
     num_fea = ln_emb.size + 1
@@ -208,17 +244,38 @@ def run(argv=None):
     if m_spa != m_den_out:
         sys.exit("ERROR: arch-sparse-feature-size " + str(m_spa) + " does not match last dim of bottom mlp "
                  + str(m_den_out))
-    nbatches = args.num_batches if args.num_batches > 0 else int(np.ceil(args.data_size / args.mini_batch_size))
-
-    # RandomDataset(reset_seed_on_access=True): numpy is re-seeded at the first batch of every epoch, and
-    # every batch is drawn in the reference's order (datagen.py; identical batches for identical flags)
     from . import datagen
 
-    train_data, _, test_data, _ = datagen.make_random_data_and_loader(args, ln_emb, m_den)
-    nbatches_test = len(test_data)
+    if bin_loader:
+        nbatches = args.num_batches if args.num_batches > 0 else len(train_ds)
+        train_data = binrecords.DeviceBatches(train_ds, device)
+        test_data = binrecords.DeviceBatches(test_ds, device)
+        test_cap = test_ds.num_records
+        order = None
 
-    def batch(j):
-        return datagen.collate_wrapper_random_offset([train_data[j]])
+        def batch(j, k):
+            # --mlperf-bin-shuffle: a new permutation of the batches every epoch, from (seed, epoch); the
+            # reference's RandomSampler draws from torch's global RNG after model construction (not reproduced)
+            nonlocal order
+            if args.mlperf_bin_shuffle and j == 0:
+                order = np.random.default_rng([args.numpy_rand_seed, k]).permutation(len(train_data))
+            return train_data[int(order[j]) if args.mlperf_bin_shuffle else j]
+
+        def test_batch(i):
+            return test_data[i]
+    else:
+        nbatches = args.num_batches if args.num_batches > 0 else int(np.ceil(args.data_size / args.mini_batch_size))
+        # RandomDataset(reset_seed_on_access=True): numpy is re-seeded at the first batch of every epoch, and
+        # every batch is drawn in the reference's order (datagen.py; identical batches for identical flags)
+        train_data, _, test_data, _ = datagen.make_random_data_and_loader(args, ln_emb, m_den)
+        test_cap = test_data.data_size
+
+        def batch(j, k):
+            return datagen.collate_wrapper_random_offset([train_data[j]])
+
+        def test_batch(i):
+            return datagen.collate_wrapper_random_offset([test_data[i]])
+    nbatches_test = len(test_data)
 
     loss_ws = np.fromstring(args.loss_weights, dtype=float, sep="-") if args.loss_function == "wbce" else None
     dlrm = DLRM_Net(m_spa, ln_emb, ln_bot, ln_top, arch_interaction_op=args.arch_interaction_op,
@@ -286,16 +343,34 @@ def run(argv=None):
         print("Saved at: epoch = {:d}/{:d}, batch = {:d}/{:d}, ntbatch = {:d}".format(
             ld_k, ld_nepochs, ld_j, ld_nbatches, ld_nbatches_test))
         print("Training state: loss = {:.6f}".format(ld_train_loss))
-        print("Testing state: accuracy = {:3.3f} %".format(ld_acc_test * 100))
+        if args.mlperf_logging:
+            print("Testing state: accuracy = {:3.3f} %, auc = {:.3f}".format(ld_acc_test * 100, ld["test_auc"]))
+        else:
+            print("Testing state: accuracy = {:3.3f} %".format(ld_acc_test * 100))
 
-    def inference(best_acc):
+    score_keys = None
+
+    def inference(best_acc, best_auc=0.0):
         """One pass over the test set (inference(), dlrm_s_pytorch.py:759-900): accuracy of round(Z) against the
-        targets, every rank's slice gathered first."""
+        targets, every rank's slice gathered first.  --mlperf-logging: the MLPerf metrics, computed on the device
+        (dlrm_b200/metrics.py); is_best is decided on the AUC against `best_auc`, and the printed best accuracy
+        is the `best_acc` passed in (the reference's behaviour)."""
+        nonlocal score_keys
+        if args.mlperf_logging:
+            from . import metrics as mlperf_metrics
+
+            if score_keys is None:
+                score_keys = mlperf_metrics.ScoreKeys(test_cap, device)
+            score_keys.reset()
         test_accu = test_samp = 0
         for i in range(nbatches_test):
             if nbatches > 0 and i >= nbatches:
                 break
-            X_t, lS_o_t, lS_i_t, T_t = datagen.collate_wrapper_random_offset([test_data[i]])
+            X_t, lS_o_t, lS_i_t, T_t = test_batch(i)
+            if args.mlperf_logging:
+                with torch.no_grad():
+                    score_keys.add(dlrm(X_t.to(device), lS_o_t, lS_i_t), T_t.to(device))
+                continue
             if world > 1 and X_t.size(0) % world != 0:
                 print("Warning: Skiping the batch %d with size %d" % (i, X_t.size(0)))
                 continue
@@ -310,6 +385,20 @@ def run(argv=None):
             S_t, T_n = Z_t.detach().cpu().numpy(), T_t.numpy()
             test_accu += np.sum((np.round(S_t, 0) == T_n).astype(np.uint8))
             test_samp += T_n.shape[0]
+        if args.mlperf_logging:
+            res = score_keys.finalize()
+            metrics = {"nepochs": args.nepochs, "nbatches": nbatches, "nbatches_test": nbatches_test,
+                       "state_dict": dlrm.state_dict(), "test_acc": res["accuracy"]}
+            is_best = res["roc_auc"] > best_auc
+            if is_best:
+                best_auc = res["roc_auc"]
+                metrics["test_auc"] = best_auc
+            print("recall {:.4f}, precision {:.4f},".format(res["recall"], res["precision"])
+                  + " f1 {:.4f}, ap {:.4f},".format(res["f1"], res["ap"])
+                  + " auc {:.4f}, best auc {:.4f},".format(res["roc_auc"], best_auc)
+                  + " accuracy {:3.3f} %, best accuracy {:3.3f} %".format(res["accuracy"] * 100, best_acc * 100),
+                  flush=True)
+            return metrics, is_best, res
         acc = test_accu / test_samp
         metrics = {"nepochs": args.nepochs, "nbatches": nbatches, "nbatches_test": nbatches_test,
                    "state_dict": dlrm.state_dict(), "test_acc": acc}
@@ -337,11 +426,14 @@ def run(argv=None):
         if args.inference_only:
             print("Testing for inference only")
             inference(best_acc_test)
+        stop = False
         for k in range(0 if not args.inference_only else args.nepochs, args.nepochs):
             if k < skip_upto_epoch:
                 continue
-            for j in range(nbatches):
-                X, lS_o, lS_i, T = batch(j)       # drawn even when skipped: the generator's order is the reference's
+            if stop:
+                break
+            for j in range(min(nbatches, len(train_data)) if bin_loader else nbatches):
+                X, lS_o, lS_i, T = batch(j, k)    # drawn even when skipped: the generator's order is the reference's
                 if j < skip_upto_batch:
                     continue
                 if world > 1 and X.size(0) % world != 0:      # dlrm_s_pytorch.py:1565-1570
@@ -391,15 +483,30 @@ def run(argv=None):
                     print("Testing at - {}/{} of epoch {},".format(j + 1, nbatches, k))
                     # (the reference does not carry the best accuracy back to this loop, :1691-1700: every test
                     #  pass that beats the LOADED accuracy saves)
-                    metrics, is_best, _ = inference(best_acc_test)
+                    metrics, is_best, res = inference(best_acc_test)
                     if is_best and args.save_model:
                         checkpoint(metrics, k, j + 1, train_loss)
                         saved = True
+                    # dlrm_b200: the thresholds act on the pass just finished and end both loops (the reference's
+                    # checks compare values its inference() never returns, :1730-1760, so they never fire)
+                    if args.mlperf_logging and 0 < args.mlperf_acc_threshold < res["accuracy"]:
+                        print("MLPerf testing accuracy threshold " + str(args.mlperf_acc_threshold)
+                              + " reached, stop training")
+                        stop = True
+                        break
+                    if args.mlperf_logging and 0 < args.mlperf_auc_threshold < res["roc_auc"]:
+                        print("MLPerf testing auc threshold " + str(args.mlperf_auc_threshold)
+                              + " reached, stop training")
+                        stop = True
+                        break
     if args.save_model and not saved and not args.inference_only:
         # dlrm_b200 addition: the reference only saves after a test pass that improved the accuracy
         # (:1703-1715); without --test-freq it would write nothing, so the final state is saved here
-        checkpoint({"nepochs": args.nepochs, "nbatches": nbatches, "nbatches_test": nbatches_test,
-                    "state_dict": dlrm.state_dict(), "test_acc": best_acc_test}, args.nepochs, 0, train_loss)
+        final = {"nepochs": args.nepochs, "nbatches": nbatches, "nbatches_test": nbatches_test,
+                 "state_dict": dlrm.state_dict(), "test_acc": best_acc_test}
+        if args.mlperf_logging:          # --load-model with --mlperf-logging reads it (the reference's best AUC: 0)
+            final["test_auc"] = 0.0
+        checkpoint(final, args.nepochs, 0, train_loss)
     if args.enable_profiling:                               # dlrm_s_pytorch.py:1795-1805
         import datetime
 

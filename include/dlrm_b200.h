@@ -482,6 +482,20 @@ int dlrm_b200_gen_multihot(void* const* out /*[host]*/, const int64_t* rows /*[h
                            uint64_t step, int64_t sample0, int64_t batch, float* X, float* target, int m_den,
                            void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * MLPerf binary records -> one packed batch (data_loader_terabyte.py:74-93 _transform_features,
+ * :229-240 CriteoBinDataset.__getitem__).  records = n int32 records [label | num_dense | num_sparse ids]:
+ *   X[b, d]            = logf((float)x + 1.0f)   (fp32 conversion, then an fp32 add; IEEE logf)
+ *   target[b]          = (float)label
+ *   indices[k*n + b]   = id mod max_ind_range (floor modulo, never negative) if max_ind_range > 0, else id
+ *   offsets[k*(n+1)+b] = k*n + b for b in 0..n   (the include_last layout of dlrm_b200/data.py)
+ * A negative id with max_ind_range <= 0 is passed through; the gather's range check reports it.
+ * n <= 0, non-positive num_dense / num_sparse or a NULL pointer is an error without a launch.
+ * ------------------------------------------------------------------------------------------ */
+int dlrm_b200_decode_records(const int32_t* records, int64_t n, int num_dense, int num_sparse,
+                             int64_t max_ind_range, float* X, float* target, int64_t* offsets,
+                             int64_t* indices, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
