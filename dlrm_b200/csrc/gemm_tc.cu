@@ -125,6 +125,12 @@ extern "C" int dlrm_b200_gemm_tc_plan_create(const dlrm_gemm_tc_desc_t* d, void*
   a.out_col = d->out_col; a.col_index = d->col_index; a.col_slab_stride = d->col_slab_stride;
   a.bias = d->bias;
   if (a.mask_act != DLRM_ACT_NONE && !a.mask_hi) { delete p; return set_error("gemm_tc: mask_act without mask_hi"); }
+  // the diverted column is stored by the fp32 store path, and every column right of it would be dropped
+  if (a.out_col && !a.out_f32) { delete p; return set_error("gemm_tc: out_col needs out_f32"); }
+  if (a.out_col && a.col_index != a.N - 1) {
+    delete p;
+    return set_error("gemm_tc: out_col diverts the last column: col_index=%lld, N=%lld", (long long)a.col_index, (long long)a.N);
+  }
   if (a.out_hi && (a.ld_out % 8)) { delete p; return set_error("gemm_tc: ld_out must be a multiple of 8"); }
   // tile width: keep >= ~64 CTAs when N is small
   const long long mt = (d->M + TC_BM - 1) / TC_BM;

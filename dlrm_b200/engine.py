@@ -1058,15 +1058,16 @@ class Engine:
         self.tc_plans = {"fwd": {}, "dgrad": {}, "wgrad": {}}
         x3 = self.tc_x3
         P = self.dense_numel
-        # split-K factors for the wgrads -> number of gradient slabs
-        self.tc_splits = {}
+        # split-K factors asked of the weight-gradient plans (upper bounds: room for that many gradient slabs);
+        # tc_splits, the slabs every reduction folds, is what each plan reports it writes
+        want_splits, self.tc_splits = {}, {}
         smax = 1
         for which in ("bot", "top"):
             ln = self.ln_bot if which == "bot" else self.ln_top
             for i in range(self.ntc[which]):
                 tiles = ((ln[i + 1] + 127) // 128) * ((ln[i] + 1 + 127) // 128)
                 sk = max(1, min(8, (120 + tiles - 1) // tiles, (B + 63) // 64))
-                self.tc_splits[(which, i)] = sk
+                want_splits[(which, i)] = sk
                 smax = max(smax, sk)
         if self.dense_grad.numel() < smax * P:
             self.dense_grad = torch.zeros(smax * P, dtype=torch.float32, device=dev)
@@ -1135,9 +1136,11 @@ class Engine:
                 self.tc_plans["wgrad"][(which, i)] = GP(
                     bwd_kb, A_hi=gh.data_ptr(), A_lo=gl.data_ptr(), lda=Np, a_mn_major=1,
                     B_hi=ih.data_ptr(), B_lo=il.data_ptr(), ldb=Kp, b_mn_major=1,
-                    M=N, N=K + 1, K=B, mode_x3=x3, split_k=self.tc_splits[(which, i)],
+                    M=N, N=K + 1, K=B, mode_x3=x3, split_k=want_splits[(which, i)],
                     out_f32=self.dense_grad.data_ptr() + oW * 4, ld_f32=K, slab_stride=P,
                     out_col=self.dense_grad.data_ptr() + ob * 4, col_index=K, col_slab_stride=P)
+                # a plan never launches an empty split: slabs past this count keep whatever an earlier step left
+                self.tc_splits[(which, i)] = self.tc_plans["wgrad"][(which, i)].info()["splits"]
                 # ---- dgrad: gz_prev = (gz W) * act'(input activation)
                 if i > 0:
                     ph, pl, Np_prev = self.tc_gz[which][i - 1]

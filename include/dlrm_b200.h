@@ -369,16 +369,21 @@ int dlrm_b200_dense_update(float* param, const float* grad, float* state /*NULL 
  * Bias: forward layers add `bias` (fp32) in the epilogue; the weight-gradient GEMMs get the bias gradient
  * for free from a constant-1 column of the activations ([dW | db] = gz^T [X | 1]).
  * Epilogue (all optional): act(); multiply by act'(y), y = mask_hi + mask_lo [M, ldmask];
- * fp32 store (split-K: one slab per split, reduced by dense_update_pack); one column diverted to
- * out_col (bias gradient); (hi, lo) bf16 stores in normal [M, ld_out] and transposed [N, ld_outT]
- * layout.  A plan holds the TMA descriptors: create once per buffer set, run every step.
+ * fp32 store (split-K: one slab per split, reduced by dense_update_pack); the last column diverted to
+ * out_col (bias gradient: needs out_f32, col_index = N - 1); (hi, lo) bf16 stores in normal [M, ld_out] and
+ * transposed [N, ld_outT] layout.  A plan holds the TMA descriptors: create once per buffer set, run every step.
+ * split_k is an upper bound: no split is left without a k block, so a plan may write fewer slabs than asked
+ * (K = 700, split_k = 8: 11 k blocks, 2 per split, 6 slabs).  plan_info reports the slabs a run writes; slabs
+ * past that count are never touched, and the caller reduces exactly that many (dlrm_dense_layer_t.num_slabs).
+ * Only operand elements inside [rows, K] are read and only output elements inside [M, N] are written: the
+ * padding up to the leading dimensions may hold anything and is left as it is.
  * ------------------------------------------------------------------------------------------ */
 typedef struct {
   const void* A_hi; const void* A_lo; int64_t lda; int a_mn_major;
   const void* B_hi; const void* B_lo; int64_t ldb; int b_mn_major;
   int64_t M, N, K;
   int mode_x3;
-  int split_k;      /* >= 1 */
+  int split_k;      /* >= 1: at most this many slabs; plan_info gives the number written */
   int tile_n;       /* 0 = auto, or 32 / 64 / 128 */
   int act;          /* DLRM_ACT_* applied to the accumulator */
   int mask_act;     /* DLRM_ACT_*: multiply by act'(y) */

@@ -228,15 +228,32 @@ def _mlp_backward(x_in, acts, layers, sigmoid_layer, g_out, dtype):
 
 def dlrm_backward(params, X, lS_o, lS_i, target, *, loss="bce", loss_ws=None, op="dot",
                   itself=False, loss_threshold=0.0, sigmoid_bot=-1, sigmoid_top=None,
-                  dtype=np.float32):
+                  dtype=np.float32, relu_masks=None):
     """Manual backprop of loss(dlrm_forward(...)).  Returns dict with
     loss, p, bot/top grads [(dW,db)], and per-table dense-by-bag grads
     ``d_ly[k]`` [B,D] (the reference's sparse COO grad has values
-    d_ly[k][bag_of(j)] at index lS_i[k][j], uncoalesced; SURVEY §8 a9)."""
+    d_ly[k][bag_of(j)] at index lS_i[k][j], uncoalesced; SURVEY §8 a9).
+
+    relu_masks = dict(bot=[y_0, ...], top=[y_0, ...]) (entries may be None): the
+    backward of ReLU layer i passes the gradient where y_i > 0 instead of where
+    this forward's own output is positive.  A checker that hands in the
+    activations of the implementation under test gets the gradient of the same
+    piecewise-linear branch, so a pre-activation within rounding of 0 is not a
+    disagreement of a whole term.  Only the backward changes: p, z and the loss
+    are this forward's own and are not recomputed, so the forward of the
+    implementation is held by whatever the checker asserts about them."""
     if sigmoid_top is None:
         sigmoid_top = len(params["top"]) - 1
     f = dlrm_forward(params, X, lS_o, lS_i, op=op, itself=itself, loss_threshold=loss_threshold,
                      sigmoid_bot=sigmoid_bot, sigmoid_top=sigmoid_top, dtype=dtype, keep=True)
+    if relu_masks is not None:
+        for name, sig in (("bot", sigmoid_bot), ("top", sigmoid_top)):
+            acts = f[name + "_acts"]
+            for i, y in enumerate(relu_masks.get(name) or []):
+                if y is not None and i != sig:
+                    # values stay this forward's (the other branch's output stands in where it is 0)
+                    acts[i] = np.where(np.asarray(y) > 0, np.where(acts[i] > 0, acts[i], y), 0).astype(dtype)
+        f["x"] = f["bot_acts"][-1]
     p, z = f["p"], f["z"]
     L = loss_forward(z, target, loss, loss_ws)
     gz = loss_backward(z, np.asarray(target, dtype=dtype), loss, loss_ws)

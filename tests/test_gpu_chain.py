@@ -17,8 +17,13 @@ def _run(use_chain, D, ln_emb, ln_bot, ln_top, B, tile_n=None, steps=2, seed=0):
 
     rng = np.random.default_rng(seed)
     params = O.random_params(rng, D, ln_emb, ln_bot, ln_top)
-    X, off, idx = O.random_batch(rng, ln_emb, B, ln_bot[0], 6)
-    tgt = np.round(rng.random((B, 1))).astype(np.float32)
+    # B may be a sequence of batch sizes stepped on ONE engine: the plans, the chain's task list and its counters
+    # are rebuilt at every change
+    batches = []
+    for b in ([B] if isinstance(B, int) else B):
+        X, off, idx = O.random_batch(rng, ln_emb, b, ln_bot[0], 6)
+        batches.append((X, off, idx, np.round(rng.random((b, 1))).astype(np.float32)))
+    B = max(b[0].shape[0] for b in batches)
     old = os.environ.get("DLRM_CHAIN_TILE_N")
     if tile_n:
         os.environ["DLRM_CHAIN_TILE_N"] = str(tile_n)
@@ -27,11 +32,12 @@ def _run(use_chain, D, ln_emb, ln_bot, ln_top, B, tile_n=None, steps=2, seed=0):
                    gemm="tc")
         e.use_chain = use_chain
         e.load_params(params)
-        sp = sparse_from_reference([torch.from_numpy(o) for o in off], [torch.from_numpy(i) for i in idx], DEV)
-        Xd, Td = torch.from_numpy(X).to(DEV), torch.from_numpy(tgt).to(DEV)
         losses = []
-        for _ in range(steps):
-            losses.append(float(e.train_step(Xd, sp, Td, 0.05, "rwsadagrad").item()))
+        for X, off, idx, tgt in batches:
+            sp = sparse_from_reference([torch.from_numpy(o) for o in off], [torch.from_numpy(i) for i in idx], DEV)
+            Xd, Td = torch.from_numpy(X).to(DEV), torch.from_numpy(tgt).to(DEV)
+            for _ in range(steps):
+                losses.append(float(e.train_step(Xd, sp, Td, 0.05, "rwsadagrad").item()))
         p = e.forward(Xd, sp).clone()
         torch.cuda.synchronize()
     finally:
@@ -55,6 +61,11 @@ CASES = [
     (128, [1000] * 4, [13, 512, 256, 128], [1024, 512, 256, 1], 2048),
     (128, [900, 700, 500], [13, 64, 128], [96, 64, 1], 300),      # ragged last m tile, narrow layers
     (16, [1000, 1000, 1000], [13, 512, 256, 64, 16], [512, 256, 1], 128),   # CFG0 shapes
+    # 11 k blocks in the weight gradients: 8 splits asked, 6 slabs written.  Both engines fold the same slabs, so these
+    # hold the chain to the per-layer path on an uneven plan and after a rebuild; which slabs to fold is
+    # tests/test_gpu_tc_batch_sequences.py's
+    (128, [1000] * 4, [13, 512, 256, 128], [1024, 512, 256, 1], 700),
+    (128, [1000] * 4, [13, 512, 256, 128], [1024, 512, 256, 1], [1024, 700]),   # plans, task list and counters rebuilt
 ]
 
 

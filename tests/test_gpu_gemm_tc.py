@@ -8,6 +8,6 @@ def test_gemm_tc_all_variants():
     from gemm_tc_check import run_all
 
     rows, txt = run_all()
-    bad = [r for r in rows if not r[3]]
+    bad = [r for r in rows if not r.ok]
     assert not bad, "wgmma GEMM mismatches:\n" + "\n".join(
-        f"{n}: err={e:.3e} tol={t:.1e} {d}" for n, e, t, _, d in bad)
+        f"{r.name}: err={r.err:.3e} tol={r.tol:.1e} {r.detail}" for r in bad)
