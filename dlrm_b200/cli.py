@@ -6,7 +6,9 @@ the hot path (datasets other than the MLPerf binary Terabyte records, QR/MD embe
 ONNX, ...) exit with the reference's style of error.  `--data-generation=dataset --mlperf-logging
 --memory-map --data-set=terabyte --mlperf-bin-loader` trains on the MLPerf binary records, decoded on
 the GPU (binrecords.DeviceBatches), and --mlperf-logging prints the reference's MLPerf metric line,
-computed on the GPU (metrics.py).  --test-freq / --inference-only run the reference's test pass (inference(),
+computed on the GPU (metrics.py).  `--data-generation=dataset --data-set={kaggle,terabyte}` without --memory-map
+trains on the preprocessed .npz with the train and test splits resident in device memory and every batch
+assembled there (criteo.DeviceBatches), in the reference's sample order.  --test-freq / --inference-only run the reference's test pass (inference(),
 :759-900), --save-model / --load-model write and read the reference's checkpoint dictionary (:860-866,
 :1399-1456, :1703-1715; a checkpoint written by the reference loads here and vice versa), --enable-profiling
 and --debug-mode do what they do there.  --max-ind-range acts on the binary records only, as in
@@ -165,15 +167,31 @@ def run(argv=None):
     # the reference's condition for its MLPerf binary loader (dlrm_data_pytorch.py:415-419); other datasets stay out
     bin_loader = (args.data_generation == "dataset" and args.mlperf_logging and args.memory_map
                   and args.data_set == "terabyte" and args.mlperf_bin_loader)
-    if args.data_generation not in ("random", "synthetic") and not bin_loader:
+    # the reference's other branch (dlrm_data_pytorch.py:518-565): the processed .npz of Kaggle or Terabyte, read whole
+    dataset = args.data_generation == "dataset" and not bin_loader
+    if dataset and args.memory_map:
+        sys.exit("ERROR: --data-generation=dataset is not supported with --memory-map outside the MLPerf binary loader "
+                 "(the per-day _reordered.npz files are not read; drop --memory-map to read the processed .npz whole, "
+                 "or use --mlperf-logging --memory-map --data-set=terabyte --mlperf-bin-loader)")
+    if dataset:
+        from . import criteo
+
+        if args.data_set not in criteo.DAYS:
+            sys.exit("ERROR: --data-set=" + args.data_set + " is not supported (kaggle | terabyte)")
+        for f in criteo.data_files(args.data_set, args.raw_data_file, args.processed_data_file):
+            if not os.path.exists(f):
+                sys.exit("ERROR: --data-generation=dataset is not supported from raw text: " + f + " does not exist "
+                         "(preprocessing is not provided: make the processed files with the reference's "
+                         "data_utils.getCriteoAdData)")
+    if args.data_generation not in ("random", "synthetic") and not (bin_loader or dataset):
         sys.exit("ERROR: --data-generation=" + args.data_generation + " is not supported (datasets are outside "
                  "the dlrm_b200 hot path; use random or synthetic, or the MLPerf binary loader: --mlperf-logging "
                  "--memory-map --data-set=terabyte --mlperf-bin-loader)")
     if args.mlperf_logging and args.mlperf_grad_accum_iter != 1:
         sys.exit("ERROR: --mlperf-grad-accum-iter=%d is not supported (1)" % args.mlperf_grad_accum_iter)
-    if args.mlperf_logging and not bin_loader and not args.round_targets:
+    if args.mlperf_logging and not (bin_loader or dataset) and not args.round_targets:
         sys.exit("ERROR: --mlperf-logging computes classification metrics: random targets need --round-targets=True")
-    if bin_loader and int(os.environ.get("WORLD_SIZE", "1")) > 1:
+    if (bin_loader or dataset) and int(os.environ.get("WORLD_SIZE", "1")) > 1:
         sys.exit("ERROR: --data-generation=dataset runs on one GPU (sharded runs need one global batch size; "
                  "test and tail batches differ)")
     if args.mlperf_logging and int(os.environ.get("WORLD_SIZE", "1")) > 1:
@@ -229,6 +247,21 @@ def run(argv=None):
         if args.max_ind_range > 0:
             ln_emb = np.minimum(ln_emb, args.max_ind_range)
         ln_bot[0] = train_ds.m_den
+    elif dataset:                                            # dlrm_s_pytorch.py:1104-1124, dlrm_data_pytorch.py:518-541
+        if args.test_mini_batch_size < 0:
+            args.test_mini_batch_size = args.mini_batch_size
+        # both constructors draw from numpy's global RNG before the model is built, as in the reference; the test
+        # split shares the train split's arrays
+        train_ds = criteo.CriteoDataset(args.data_set, args.max_ind_range, args.data_sub_sample_rate,
+                                        args.data_randomize, "train", args.raw_data_file, args.processed_data_file,
+                                        False, args.dataset_multiprocessing)
+        test_ds = criteo.CriteoDataset(args.data_set, args.max_ind_range, args.data_sub_sample_rate,
+                                       args.data_randomize, "test", args.raw_data_file, args.processed_data_file,
+                                       False, args.dataset_multiprocessing, data=train_ds)
+        ln_emb = np.asarray(train_ds.counts)
+        if args.max_ind_range > 0:
+            ln_emb = np.minimum(ln_emb, args.max_ind_range)
+        ln_bot[0] = train_ds.m_den
     else:
         ln_emb = np.fromstring(args.arch_embedding_size, dtype=int, sep="-")
     m_den = ln_bot[0]
@@ -260,6 +293,19 @@ def run(argv=None):
             if args.mlperf_bin_shuffle and j == 0:
                 order = np.random.default_rng([args.numpy_rand_seed, k]).permutation(len(train_data))
             return train_data[int(order[j]) if args.mlperf_bin_shuffle else j]
+
+        def test_batch(i):
+            return test_data[i]
+    elif dataset:
+        # the splits stay in device memory; every batch is assembled there (criteo.DeviceBatches), in file or
+        # pre-shuffled order, the same every epoch (the reference's DataLoader has shuffle=False)
+        train_data = criteo.DeviceBatches(train_ds, args.mini_batch_size, device)
+        test_data = criteo.DeviceBatches(test_ds, args.test_mini_batch_size, device)
+        nbatches = args.num_batches if args.num_batches > 0 else len(train_data)
+        test_cap = len(test_ds)
+
+        def batch(j, k):
+            return train_data[j]
 
         def test_batch(i):
             return test_data[i]
@@ -382,7 +428,7 @@ def run(argv=None):
                 parts = [torch.empty_like(Z_t) for _ in range(world)]
                 tdist.all_gather(parts, Z_t.contiguous())
                 Z_t = torch.cat(parts)
-            S_t, T_n = Z_t.detach().cpu().numpy(), T_t.numpy()
+            S_t, T_n = Z_t.detach().cpu().numpy(), T_t.cpu().numpy()
             test_accu += np.sum((np.round(S_t, 0) == T_n).astype(np.uint8))
             test_samp += T_n.shape[0]
         if args.mlperf_logging:
@@ -432,7 +478,7 @@ def run(argv=None):
                 continue
             if stop:
                 break
-            for j in range(min(nbatches, len(train_data)) if bin_loader else nbatches):
+            for j in range(min(nbatches, len(train_data)) if (bin_loader or dataset) else nbatches):
                 X, lS_o, lS_i, T = batch(j, k)    # drawn even when skipped: the generator's order is the reference's
                 if j < skip_upto_batch:
                     continue

@@ -42,7 +42,76 @@ __global__ void __launch_bounds__(256) decode_records_kernel(const int32_t* __re
   }
 }
 
+// Batch assembly from a split resident in device memory (dlrm_data_pytorch.py:293-296 __getitem__ + :324-337
+// collate_wrapper_criteo_offset): sample b of the batch is row ids[b] of X_int [N, nd], X_cat [N, ns], y [N].
+// One block per tile of GATHER_TILE samples.  The ids of a shuffled split point at random rows, so each row is
+// read as a run of consecutive words (coalesced) into a shared-memory tile, which is then written out the way
+// decode_records_kernel writes it: X and target row-major, ids table-major (coalesced along the batch).
+constexpr int GATHER_TILE = 64;
+constexpr int GATHER_THREADS = 256;
+
+__device__ __forceinline__ long long fold_id(long long id, long long max_ind_range) {
+  if (max_ind_range > 0) {  // floor modulo (Python / torch `%`): never negative
+    id %= max_ind_range;
+    if (id < 0) id += max_ind_range;
+  }
+  return id;
+}
+
+__global__ void __launch_bounds__(GATHER_THREADS) gather_records_kernel(
+    const int32_t* __restrict__ X_int, const int32_t* __restrict__ X_cat, const int32_t* __restrict__ y,
+    const long long* __restrict__ ids, long long n, int nd, int ns, long long max_ind_range,
+    float* __restrict__ X, float* __restrict__ target, long long* __restrict__ offsets,
+    long long* __restrict__ indices) {
+  extern __shared__ int32_t tile[];  // [GATHER_TILE][pitch]: nd dense words, ns ids, the label
+  const int words = nd + ns + 1;
+  const int pitch = words | 1;       // odd pitch: the column reads of the write phase are conflict-free
+  const long long b0 = (long long)blockIdx.x * GATHER_TILE;
+  const int m = (int)min((long long)GATHER_TILE, n - b0);
+  for (int t = threadIdx.x; t < m * words; t += GATHER_THREADS) {
+    const int s = t / words, w = t - s * words;
+    const long long r = ids[b0 + s];
+    tile[s * pitch + w] = w < nd ? X_int[r * nd + w] : w < nd + ns ? X_cat[r * ns + (w - nd)] : y[r];
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < m * nd; t += GATHER_THREADS) {
+    const int s = t / nd, d = t - s * nd;
+    // fp32 conversion first, then the add in fp32: torch.log(torch.tensor(x, dtype=torch.float) + 1)
+    X[(b0 + s) * nd + d] = logf(__fadd_rn(__int2float_rn(tile[s * pitch + d]), 1.0f));
+  }
+  for (int t = threadIdx.x; t < ns * GATHER_TILE; t += GATHER_THREADS) {
+    const int k = t / GATHER_TILE, s = t - k * GATHER_TILE;
+    if (s < m) indices[(long long)k * n + b0 + s] = fold_id(tile[s * pitch + nd + k], max_ind_range);
+  }
+  if (threadIdx.x < m) target[b0 + threadIdx.x] = (float)tile[threadIdx.x * pitch + nd + ns];
+  for (long long o = (long long)blockIdx.x * GATHER_THREADS + threadIdx.x; o < (long long)ns * (n + 1);
+       o += (long long)gridDim.x * GATHER_THREADS)
+    offsets[o] = o - o / (n + 1);  // k*(n+1) + b  ->  k*n + b
+}
+
 }  // namespace dlrm
+
+extern "C" int dlrm_b200_gather_records(const int32_t* X_int, const int32_t* X_cat, const int32_t* y,
+                                        const int64_t* ids, int64_t n, int num_dense, int num_sparse,
+                                        int64_t max_ind_range, float* X, float* target, int64_t* offsets,
+                                        int64_t* indices, void* stream) {
+  using namespace dlrm;
+  if (n <= 0) return set_error("gather_records: n=%lld samples (must be > 0)", (long long)n);
+  if (num_dense <= 0 || num_sparse <= 0 || num_dense + num_sparse + 1 > 128)
+    return set_error("gather_records: num_dense=%d, num_sparse=%d (both > 0, at most 127 words per sample)",
+                     num_dense, num_sparse);
+  if (!X_int || !X_cat || !y || !ids || !X || !target || !offsets || !indices)
+    return set_error("gather_records: NULL pointer");
+  const long long blocks = (n + GATHER_TILE - 1) / GATHER_TILE;
+  if (blocks >= (1ll << 31)) return set_error("gather_records: %lld samples is too many for one call", (long long)n);
+  const size_t smem = sizeof(int32_t) * GATHER_TILE * ((num_dense + num_sparse + 1) | 1);
+  gather_records_kernel<<<(unsigned)blocks, GATHER_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
+      X_int, X_cat, y, reinterpret_cast<const long long*>(ids), (long long)n, num_dense, num_sparse,
+      (long long)max_ind_range, X, target, reinterpret_cast<long long*>(offsets),
+      reinterpret_cast<long long*>(indices));
+  DLRM_CHECK_LAUNCH("gather_records_kernel");
+  return 0;
+}
 
 extern "C" int dlrm_b200_decode_records(const int32_t* records, int64_t n, int num_dense, int num_sparse,
                                         int64_t max_ind_range, float* X, float* target, int64_t* offsets,

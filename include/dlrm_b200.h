@@ -501,6 +501,19 @@ int dlrm_b200_decode_records(const int32_t* records, int64_t n, int num_dense, i
                              int64_t max_ind_range, float* X, float* target, int64_t* offsets,
                              int64_t* indices, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * One packed batch from a processed Criteo split resident in device memory (dlrm_data_pytorch.py:293-296
+ * CriteoDataset.__getitem__, :324-337 collate_wrapper_criteo_offset).  X_int [N, num_dense], X_cat
+ * [N, num_sparse] and y [N] are int32 row-major; sample b of the batch is row ids[b] (int64 [n], device).
+ * The outputs are exactly those of dlrm_b200_decode_records for the records [y | X_int | X_cat] of rows
+ * ids[0..n).  The ids are not checked: the caller guarantees 0 <= ids[b] < N.
+ * n <= 0, non-positive num_dense / num_sparse, more than 127 words per sample or a NULL pointer is an
+ * error without a launch.
+ * ------------------------------------------------------------------------------------------ */
+int dlrm_b200_gather_records(const int32_t* X_int, const int32_t* X_cat, const int32_t* y, const int64_t* ids,
+                             int64_t n, int num_dense, int num_sparse, int64_t max_ind_range, float* X,
+                             float* target, int64_t* offsets, int64_t* indices, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
