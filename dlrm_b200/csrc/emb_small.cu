@@ -238,6 +238,8 @@ extern "C" int dlrm_b200_emb_bwd_small_update(const dlrm_emb_bwd_table_t* tables
   if (dim <= 0 || dim % 4 || dim > 512) return set_error("emb_bwd_small_update: dim=%d (multiple of 4, <= 512)", dim);
   if (!tables || !scratch || (!dY && !peer_dY)) return set_error("emb_bwd_small_update: NULL pointer");
   if (dy_stride_sample % 4) return set_error("emb_bwd_small_update: dY rows must be 16-byte aligned");
+  // the accumulate kernel reads every dY row with float4 loads: the base pointer(s) must be 16-byte aligned too
+  if (!peer_dY && !aligned16(dY)) return set_error("emb_bwd_small_update: dY must be 16-byte aligned");
   const int dtype = tables[0].weight_dtype;
   if (dtype != DLRM_DTYPE_F32 && dtype != DLRM_DTYPE_F16) return set_error("emb_bwd_small_update: weight_dtype=%d", dtype);
   if (dtype == DLRM_DTYPE_F16 && dim % 8) return set_error("emb_bwd_small_update: fp16 tables need dim %% 8 == 0 (dim=%d)", dim);
@@ -278,6 +280,7 @@ extern "C" int dlrm_b200_emb_bwd_small_update(const dlrm_emb_bwd_table_t* tables
       return set_error("emb_bwd_small_update: world=%d batch_local=%lld batch=%lld", world, (long long)batch_local, (long long)batch);
     for (int d = 0; d < world; ++d) {
       if (!peer_dY[d]) return set_error("emb_bwd_small_update: peer %d pointer is NULL", d);
+      if (!aligned16(peer_dY[d])) return set_error("emb_bwd_small_update: peer %d dY must be 16-byte aligned", d);
       P.peer_dY[d] = peer_dY[d];
     }
     P.peer_batch = batch_local;

@@ -462,7 +462,9 @@ int dlrm_b200_emb_bag_fwd_remote(const dlrm_emb_remote_table_t* tables /*[host]*
  * two-pass coalesce + row update instead of the per-row list walk (csrc/emb_small.cu).  Same semantics as
  * dlrm_b200_emb_bwd_update (grad.coalesce() + optim/rwsadagrad.py:117-143 / sparse SGD), deterministic.
  * Every table needs use_dy_off; `scratch` holds the per-chunk partial sums
- * (dlrm_b200_emb_bwd_small_scratch_bytes(total rows of the call, dim, batch) bytes). */
+ * (dlrm_b200_emb_bwd_small_scratch_bytes(total rows of the call, dim, batch) bytes).
+ * dY (or every peer_dY[d], d < world) must be 16-byte aligned and dy_stride_sample / dy_off multiples of 4:
+ * otherwise an error without a launch (the rows are read with 16-byte loads; there is no scalar kernel). */
 int64_t dlrm_b200_emb_bwd_small_scratch_bytes(int64_t total_small_rows, int dim, int64_t batch);
 int dlrm_b200_emb_bwd_small_update(const dlrm_emb_bwd_table_t* tables /*[host]*/, int num_tables, int dim,
                                    int64_t batch, int idx_bytes, int include_last, const float* dY,
