@@ -84,7 +84,7 @@ SYMBOLS = [
     "dlrm_b200_gemm_chain_run", "dlrm_b200_gemm_chain_destroy", "dlrm_b200_gemm_chain_set_trace",
     "dlrm_b200_emb_bwd_small_scratch_bytes", "dlrm_b200_emb_bwd_small_update", "dlrm_b200_emb_reduce_partials",
     "dlrm_b200_block_copy", "dlrm_b200_gen_multihot", "dlrm_b200_set_tunable", "dlrm_b200_emb_bag_fwd_remote", "dlrm_b200_split_bf16", "dlrm_b200_dense_update_pack",
-    "dlrm_b200_decode_records", "dlrm_b200_gather_records",
+    "dlrm_b200_decode_records", "dlrm_b200_gather_records", "dlrm_b200_ingest_records",
 ]
 
 
@@ -148,6 +148,7 @@ def _declare(lib):
     lib.dlrm_b200_dense_update_pack.argtypes = [C.POINTER(DenseLayer), i32, i32, f32, f32, vp]
     lib.dlrm_b200_decode_records.argtypes = [vp, i64, i32, i32, i64, vp, vp, vp, vp, vp]
     lib.dlrm_b200_gather_records.argtypes = [vp, vp, vp, vp, i64, i32, i32, i64, vp, vp, vp, vp, vp]
+    lib.dlrm_b200_ingest_records.argtypes = [vp, i32, vp, i32, vp, i32, i64, i32, i32, vp, vp, vp, i64, i64, vp, vp]
     for name in SYMBOLS:
         fn = getattr(lib, name)
         if name in ("dlrm_b200_head_scratch_bytes", "dlrm_b200_emb_bwd_small_scratch_bytes"):

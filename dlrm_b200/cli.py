@@ -8,8 +8,9 @@ ONNX, ...) exit with the reference's style of error.  `--data-generation=dataset
 the GPU (binrecords.DeviceBatches), and --mlperf-logging prints the reference's MLPerf metric line,
 computed on the GPU (metrics.py).  `--data-generation=dataset --data-set={kaggle,terabyte}` without --memory-map
 trains on the preprocessed .npz with the train and test splits resident in device memory and every batch
-assembled there (criteo.DeviceBatches), in the reference's sample order.  --test-freq / --inference-only run the reference's test pass (inference(),
-:759-900), --save-model / --load-model write and read the reference's checkpoint dictionary (:860-866,
+assembled there (criteo.DeviceBatches), in the reference's sample order; with --memory-map (outside the binary
+loader) it trains on the per-day *_reordered.npz files, streamed through a device ring (criteo_days.DayBatches).
+--test-freq / --inference-only run the reference's test pass (inference(), :759-900), --save-model / --load-model write and read the reference's checkpoint dictionary (:860-866,
 :1399-1456, :1703-1715; a checkpoint written by the reference loads here and vice versa), --enable-profiling
 and --debug-mode do what they do there.  --max-ind-range acts on the binary records only, as in
 the reference; --mlperf-grad-accum-iter other than 1 is rejected.  The random-data generator draws from numpy's global RNG in EXACTLY the
@@ -169,15 +170,25 @@ def run(argv=None):
                   and args.data_set == "terabyte" and args.mlperf_bin_loader)
     # the reference's other branch (dlrm_data_pytorch.py:518-565): the processed .npz of Kaggle or Terabyte, read whole
     dataset = args.data_generation == "dataset" and not bin_loader
-    if dataset and args.memory_map:
-        sys.exit("ERROR: --data-generation=dataset is not supported with --memory-map outside the MLPerf binary loader "
-                 "(the per-day _reordered.npz files are not read; drop --memory-map to read the processed .npz whole, "
-                 "or use --mlperf-logging --memory-map --data-set=terabyte --mlperf-bin-loader)")
+    # --memory-map: the per-day *_reordered.npz files, streamed through device memory (dlrm_data_pytorch.py:93-199,
+    # :474-517); both reference loaders of this path give the same batches
+    days = dataset and args.memory_map
     if dataset:
         from . import criteo
 
         if args.data_set not in criteo.DAYS:
             sys.exit("ERROR: --data-set=" + args.data_set + " is not supported (kaggle | terabyte)")
+    if days:
+        from . import criteo_days
+
+        day_files, count_file, fea_file = criteo_days.day_files(args.data_set, args.raw_data_file)
+        for f in day_files + [count_file, fea_file]:
+            if not os.path.exists(f):
+                sys.exit("ERROR: --data-generation=dataset is not supported from raw text with --memory-map: " + f
+                         + " does not exist, and without it the per-day _reordered.npz files are not read "
+                         "(preprocessing is not provided: make them with the reference's data_utils.getCriteoAdData "
+                         "and --memory-map)")
+    elif dataset:
         for f in criteo.data_files(args.data_set, args.raw_data_file, args.processed_data_file):
             if not os.path.exists(f):
                 sys.exit("ERROR: --data-generation=dataset is not supported from raw text: " + f + " does not exist "
@@ -247,6 +258,20 @@ def run(argv=None):
         if args.max_ind_range > 0:
             ln_emb = np.minimum(ln_emb, args.max_ind_range)
         ln_bot[0] = train_ds.m_den
+    elif days:                                               # dlrm_data_pytorch.py:93-199, :474-517
+        if args.test_mini_batch_size < 0:
+            args.test_mini_batch_size = args.mini_batch_size
+        # the reference builds a train and a test CriteoDataset(memory_map=True); neither draws from numpy's RNG
+        for _ in range(2):
+            print("Reading pre-processed data=%s" % args.processed_data_file)
+            print("Sparse features= %d, Dense features= %d" % (criteo.SPA_FEA, criteo.DEN_FEA))
+        with np.load(fea_file) as d:
+            ln_emb = np.asarray(d["counts"])
+        if len(ln_emb) != criteo.SPA_FEA:
+            sys.exit("ERROR: " + fea_file + " holds %d counts (26)" % len(ln_emb))
+        if args.max_ind_range > 0:
+            ln_emb = np.minimum(ln_emb, args.max_ind_range)
+        ln_bot[0] = criteo.DEN_FEA
     elif dataset:                                            # dlrm_s_pytorch.py:1104-1124, dlrm_data_pytorch.py:518-541
         if args.test_mini_batch_size < 0:
             args.test_mini_batch_size = args.mini_batch_size
@@ -293,6 +318,24 @@ def run(argv=None):
             if args.mlperf_bin_shuffle and j == 0:
                 order = np.random.default_rng([args.numpy_rand_seed, k]).permutation(len(train_data))
             return train_data[int(order[j]) if args.mlperf_bin_shuffle else j]
+
+        def test_batch(i):
+            return test_data[i]
+    elif days:
+        # every batch is assembled on the GPU from a device ring the day files stream through (criteo_days.py);
+        # a new epoch or test pass restarts its stream at day 0
+        try:
+            train_data = criteo_days.DayBatches(args.data_set, args.raw_data_file, "train", args.mini_batch_size,
+                                                args.max_ind_range, device)
+            test_data = criteo_days.DayBatches(args.data_set, args.raw_data_file, "test", args.test_mini_batch_size,
+                                               args.max_ind_range, device)
+        except ValueError as e:
+            sys.exit("ERROR: " + str(e))
+        nbatches = args.num_batches if args.num_batches > 0 else len(train_data)
+        test_cap = test_data.num_samples
+
+        def batch(j, k):
+            return train_data[j]
 
         def test_batch(i):
             return test_data[i]
@@ -479,6 +522,8 @@ def run(argv=None):
             if stop:
                 break
             for j in range(min(nbatches, len(train_data)) if (bin_loader or dataset) else nbatches):
+                if days and j < skip_upto_batch:
+                    continue                      # the day stream seeks to the first batch it trains on
                 X, lS_o, lS_i, T = batch(j, k)    # drawn even when skipped: the generator's order is the reference's
                 if j < skip_upto_batch:
                     continue
@@ -545,6 +590,9 @@ def run(argv=None):
                               + " reached, stop training")
                         stop = True
                         break
+    if days:                                                # the inflate threads end with the run
+        train_data.close()
+        test_data.close()
     if args.save_model and not saved and not args.inference_only:
         # dlrm_b200 addition: the reference only saves after a test pass that improved the accuracy
         # (:1703-1715); without --test-freq it would write nothing, so the final state is saved here

@@ -89,6 +89,69 @@ __global__ void __launch_bounds__(GATHER_THREADS) gather_records_kernel(
     offsets[o] = o - o / (n + 1);  // k*(n+1) + b  ->  k*n + b
 }
 
+
+// Per-day Criteo chunks (the reference's `*_{d}_reordered.npz`, dlrm_data_pytorch.py:270-289) into a device ring of
+// int32 rows: one thread per element of the chunk, members in order X_int [n, nd], X_cat [n, ns], y [n], each in
+// the dtype its file stores.  Row r goes to ring row (dst + r) mod capacity.  A value that is not an exact integer
+// in int32 range, a negative id or a label outside {0, 1} is not written; the smallest `r * 4 + member` of such
+// values is kept in *bad (atomicMin), so the host learns the first bad row and which member holds it.
+enum : int { INGEST_F64 = 0, INGEST_I64 = 1, INGEST_I32 = 2 };
+
+__device__ __forceinline__ bool ingest_load(const void* p, int dtype, long long i, int32_t* out) {
+  if (dtype == INGEST_I32) {
+    *out = static_cast<const int32_t*>(p)[i];
+    return true;
+  }
+  if (dtype == INGEST_I64) {
+    const long long v = static_cast<const long long*>(p)[i];
+    *out = (int32_t)v;
+    return v >= INT32_MIN && v <= INT32_MAX;
+  }
+  const double v = static_cast<const double*>(p)[i];
+  // NaN fails both comparisons; inside the range the cast is exact iff v has no fraction
+  if (!(v >= -2147483648.0 && v <= 2147483647.0)) return false;
+  *out = (int32_t)v;
+  return (double)*out == v;
+}
+
+__global__ void __launch_bounds__(256) ingest_records_kernel(
+    const void* __restrict__ x_int, int int_dtype, const void* __restrict__ x_cat, int cat_dtype,
+    const void* __restrict__ y, int y_dtype, long long n, int nd, int ns, int32_t* __restrict__ ring_int,
+    int32_t* __restrict__ ring_cat, int32_t* __restrict__ ring_y, long long capacity, long long dst,
+    unsigned long long* __restrict__ bad) {
+  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long n_int = n * nd, n_cat = n * ns;
+  int member, w;
+  long long r, i;
+  const void* src;
+  int dtype;
+  if (e < n_int) {
+    member = 0, src = x_int, dtype = int_dtype, i = e, r = e / nd, w = (int)(e - r * nd);
+  } else if (e < n_int + n_cat) {
+    member = 1, src = x_cat, dtype = cat_dtype, i = e - n_int, r = i / ns, w = (int)(i - r * ns);
+  } else if (e < n_int + n_cat + n) {
+    member = 2, src = y, dtype = y_dtype, i = e - n_int - n_cat, r = i, w = 0;
+  } else {
+    return;
+  }
+  int32_t v;
+  bool ok = ingest_load(src, dtype, i, &v);
+  if (member == 1) ok = ok && v >= 0;
+  if (member == 2) ok = ok && (v == 0 || v == 1);
+  if (!ok) {
+    atomicMin(bad, (unsigned long long)(r * 4 + member));
+    return;
+  }
+  long long row = dst + r;
+  if (row >= capacity) row -= capacity;
+  if (member == 0)
+    ring_int[row * nd + w] = v;
+  else if (member == 1)
+    ring_cat[row * ns + w] = v;
+  else
+    ring_y[row] = v;
+}
+
 }  // namespace dlrm
 
 extern "C" int dlrm_b200_gather_records(const int32_t* X_int, const int32_t* X_cat, const int32_t* y,
@@ -128,5 +191,32 @@ extern "C" int dlrm_b200_decode_records(const int32_t* records, int64_t n, int n
       records, (long long)n, num_dense, num_sparse, (long long)max_ind_range, X, target,
       reinterpret_cast<long long*>(offsets), reinterpret_cast<long long*>(indices));
   DLRM_CHECK_LAUNCH("decode_records_kernel");
+  return 0;
+}
+
+extern "C" int dlrm_b200_ingest_records(const void* x_int, int x_int_dtype, const void* x_cat, int x_cat_dtype,
+                                        const void* y, int y_dtype, int64_t n, int num_dense, int num_sparse,
+                                        int32_t* ring_int, int32_t* ring_cat, int32_t* ring_y, int64_t capacity,
+                                        int64_t dst, uint64_t* bad, void* stream) {
+  using namespace dlrm;
+  if (n <= 0 || n > capacity)
+    return set_error("ingest_records: n=%lld rows for a ring of %lld (must be in 1..capacity)", (long long)n,
+                     (long long)capacity);
+  if (dst < 0 || dst >= capacity)
+    return set_error("ingest_records: dst=%lld outside the ring [0, %lld)", (long long)dst, (long long)capacity);
+  if (num_dense <= 0 || num_sparse <= 0)
+    return set_error("ingest_records: num_dense=%d, num_sparse=%d (both must be > 0)", num_dense, num_sparse);
+  for (int d : {x_int_dtype, x_cat_dtype, y_dtype})
+    if (d != INGEST_F64 && d != INGEST_I64 && d != INGEST_I32)
+      return set_error("ingest_records: dtype code %d (0 float64, 1 int64, 2 int32)", d);
+  if (!x_int || !x_cat || !y || !ring_int || !ring_cat || !ring_y || !bad)
+    return set_error("ingest_records: NULL pointer");
+  const long long total = n * (1ll + num_dense + num_sparse);
+  const long long blocks = (total + 255) / 256;
+  if (blocks >= (1ll << 31)) return set_error("ingest_records: %lld rows is too many for one call", (long long)n);
+  ingest_records_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      x_int, x_int_dtype, x_cat, x_cat_dtype, y, y_dtype, (long long)n, num_dense, num_sparse, ring_int, ring_cat,
+      ring_y, (long long)capacity, (long long)dst, reinterpret_cast<unsigned long long*>(bad));
+  DLRM_CHECK_LAUNCH("ingest_records_kernel");
   return 0;
 }

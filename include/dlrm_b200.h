@@ -516,6 +516,25 @@ int dlrm_b200_gather_records(const int32_t* X_int, const int32_t* X_cat, const i
                              int64_t n, int num_dense, int num_sparse, int64_t max_ind_range, float* X,
                              float* target, int64_t* offsets, int64_t* indices, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * One chunk of a per-day Criteo file (the reference's `*_{d}_reordered.npz`, read with --memory-map) into a
+ * device ring of int32 rows.  x_int [n, num_dense], x_cat [n, num_sparse] and y [n] are row-major device arrays
+ * in the dtype the file stores: 0 float64, 1 int64, 2 int32.  Chunk row r goes to ring row
+ * (dst + r) mod capacity of ring_int [capacity, num_dense], ring_cat [capacity, num_sparse], ring_y [capacity];
+ * no other ring row is written.
+ * Every value is checked: an exact integer inside int32 range, and in addition an id >= 0 and a label in {0, 1}.
+ * A value that fails is not written, and *bad (device) becomes min(*bad, r * 4 + member), member 0 X_int,
+ * 1 X_cat, 2 y: the caller sets *bad to UINT64_MAX first and reads it once the chunk's work has completed.
+ * Rows whose values all pass are converted exactly, so dlrm_b200_gather_records over ring rows gives the
+ * reference's collate of the same samples.
+ * n outside 1..capacity, dst outside [0, capacity), non-positive num_dense / num_sparse, an unknown dtype code
+ * or a NULL pointer is an error without a launch.
+ * ------------------------------------------------------------------------------------------ */
+int dlrm_b200_ingest_records(const void* x_int, int x_int_dtype, const void* x_cat, int x_cat_dtype, const void* y,
+                             int y_dtype, int64_t n, int num_dense, int num_sparse, int32_t* ring_int,
+                             int32_t* ring_cat, int32_t* ring_y, int64_t capacity, int64_t dst, uint64_t* bad,
+                             void* stream);
+
 #ifdef __cplusplus
 }
 #endif
