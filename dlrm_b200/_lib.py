@@ -14,8 +14,7 @@ LOSS_MSE, LOSS_BCE, LOSS_WBCE = 0, 1, 2
 OPT_SGD, OPT_RWSADAGRAD, OPT_ADAGRAD = 0, 1, 2
 GEMM_SIMT_FP32, GEMM_TC_BF16X3, GEMM_TC_BF16 = 0, 1, 2
 DTYPE_F32, DTYPE_F16 = 0, 1
-TUNE = dict(emb_bags_per_group=0, emb_unroll=1, emb_block=2, upd_block=3, gemm_splitk=4, gemm_smem_kb=5,
-            head_rows=6, interact_bwd_cols=7, pdl=8, chain_order=9, upd_lean=10, upd_debug=11)
+TUNE = dict(emb_bags_per_group=0, emb_unroll=1, head_rows=6, interact_bwd_cols=7, pdl=8, upd_lean=10, upd_debug=11)
 
 
 class EmbFwdTable(C.Structure):
@@ -80,8 +79,7 @@ SYMBOLS = [
     "dlrm_b200_interact_fwd", "dlrm_b200_interact_bwd", "dlrm_b200_loss_fwd_bwd",
     "dlrm_b200_dense_update",
     "dlrm_b200_gemm_tc_plan_create", "dlrm_b200_gemm_tc_plan_info", "dlrm_b200_gemm_tc_run",
-    "dlrm_b200_gemm_tc_plan_destroy", "dlrm_b200_gemm_chain_create", "dlrm_b200_gemm_chain_info",
-    "dlrm_b200_gemm_chain_run", "dlrm_b200_gemm_chain_destroy", "dlrm_b200_gemm_chain_set_trace",
+    "dlrm_b200_gemm_tc_plan_destroy",
     "dlrm_b200_emb_bwd_small_scratch_bytes", "dlrm_b200_emb_bwd_small_update", "dlrm_b200_emb_reduce_partials",
     "dlrm_b200_block_copy", "dlrm_b200_gen_multihot", "dlrm_b200_set_tunable", "dlrm_b200_emb_bag_fwd_remote", "dlrm_b200_split_bf16", "dlrm_b200_dense_update_pack",
     "dlrm_b200_decode_records", "dlrm_b200_gather_records", "dlrm_b200_ingest_records",
@@ -130,10 +128,6 @@ def _declare(lib):
     lib.dlrm_b200_gemm_tc_plan_create.argtypes = [C.POINTER(GemmTcDesc), C.POINTER(vp)]
     lib.dlrm_b200_gemm_tc_plan_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
     lib.dlrm_b200_gemm_tc_run.argtypes = [vp, vp]
-    lib.dlrm_b200_gemm_chain_create.argtypes = [C.POINTER(vp), C.POINTER(i32), C.POINTER(i32), i32, vp, i64, C.POINTER(vp)]
-    lib.dlrm_b200_gemm_chain_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
-    lib.dlrm_b200_gemm_chain_run.argtypes = [vp, vp]
-    lib.dlrm_b200_gemm_chain_set_trace.argtypes = [vp, vp]
     lib.dlrm_b200_emb_bwd_small_scratch_bytes.argtypes = [i64, i32, i64]
     lib.dlrm_b200_emb_bwd_small_update.argtypes = [C.POINTER(EmbBwdTable), i32, i32, i64, i32, i32, vp, C.POINTER(vp), i32,
                                                    i64, i64, i32, f32, f32, vp, i64, vp]
@@ -142,7 +136,6 @@ def _declare(lib):
     lib.dlrm_b200_block_copy.argtypes = [C.POINTER(vp), C.POINTER(vp), C.POINTER(i64), i32, vp]
     lib.dlrm_b200_gen_multihot.argtypes = [C.POINTER(vp), C.POINTER(i64), C.POINTER(i32), C.POINTER(i32), i32, i32,
                                            C.c_uint64, C.c_uint64, i64, i64, vp, vp, i32, vp]
-    lib.dlrm_b200_gemm_chain_destroy.argtypes = [vp]
     lib.dlrm_b200_gemm_tc_plan_destroy.argtypes = [vp]
     lib.dlrm_b200_split_bf16.argtypes = [vp, i64, i64, i64, vp, vp, i64, vp]
     lib.dlrm_b200_dense_update_pack.argtypes = [C.POINTER(DenseLayer), i32, i32, f32, f32, vp]
@@ -226,44 +219,3 @@ class GemmTcPlan:
         except Exception:
             pass
 
-
-class GemmChain:
-    """A whole MLP chain (list of GemmTcPlan + producer/consumer dependencies) as ONE persistent launch
-    (csrc/gemm_chain.cu).  `counters` is a zeroed int32 device tensor owned by the caller."""
-
-    def __init__(self, plans, dep, dep_on_k, counters):
-        self.plans = list(plans)            # keep the plans (TMA descriptors are copied, buffers are not) alive
-        self.counters = counters
-        n = len(self.plans)
-        arr = (C.c_void_p * n)(*[p.handle.value for p in self.plans])
-        d = (C.c_int * n)(*[int(v) for v in dep])
-        k = (C.c_int * n)(*[int(v) for v in dep_on_k])
-        self.handle = C.c_void_p()
-        check(lib().dlrm_b200_gemm_chain_create(arr, d, k, n, counters.data_ptr(), counters.numel(),
-                                                C.byref(self.handle)), "gemm_chain_create")
-
-    @staticmethod
-    def counters_needed(plans):
-        return 2 + sum((int(p.desc.M) + 127) // 128 for p in plans)
-
-    def info(self):
-        a, b, c, e = C.c_int(), C.c_int(), C.c_int(), C.c_int()
-        check(lib().dlrm_b200_gemm_chain_info(self.handle, C.byref(a), C.byref(b), C.byref(c), C.byref(e)))
-        return dict(tasks=a.value, ctas=b.value, stages=c.value, smem=e.value)
-
-    def run(self, stream):
-        check(lib().dlrm_b200_gemm_chain_run(self.handle, stream), "gemm_chain_run")
-
-    def set_trace(self, trace):
-        """trace: uint64/int64 device tensor [tasks, 8] (or None to switch tracing off)."""
-        self._trace = trace
-        check(lib().dlrm_b200_gemm_chain_set_trace(self.handle, trace.data_ptr() if trace is not None else None),
-              "gemm_chain_set_trace")
-
-    def __del__(self):
-        try:
-            if self.handle:
-                lib().dlrm_b200_gemm_chain_destroy(self.handle)
-                self.handle = None
-        except Exception:
-            pass

@@ -17,19 +17,14 @@ int get_tunable(int id);
 // outside its table.  Kernels only set bits; dlrm_b200_check_device_errors() reads and clears it.
 unsigned* err_word_device();
 
-enum Tunable {
+enum Tunable {   // ids are what dlrm_b200_set_tunable takes: a retired id is left unused, not reassigned
   TUNE_EMB_BAGS_PER_GROUP = 0,  // bags processed back to back by one lane group
   TUNE_EMB_UNROLL = 1,          // rows in flight per lane group (4 or 8)
-  TUNE_EMB_BLOCK = 2,           // threads per CTA in the gather
-  TUNE_UPD_BLOCK = 3,
-  TUNE_GEMM_SPLITK = 4,
-  TUNE_GEMM_SMEM_KB = 5,        // operand-ring budget per GEMM CTA at plan creation (0 = 200 KB, the deepest ring)
   TUNE_HEAD_ROWS = 6,           // samples per CTA in the fused head (16 or 32; 0 = default)
   TUNE_INTERACT_BWD_COLS = 7,   // 1 = one column per thread (first kernel), else float2 columns
   TUNE_PDL = 8,                 // programmatic dependent launch on the dense chain: 0/1 = on, 2 = off
   TUNE_UPD_LEAN = 10,           // embedding update, dim <= 128: 2 = the general kernel instead of the lean one
   TUNE_UPD_DEBUG = 11,          // timing experiments on the update kernel (see EmbBwdParams::debug); 0 = off
-  TUNE_CHAIN_ORDER = 9,         // gemm_chain task order: 0/1 = layer by layer, 2 = m-tile major across layers
   TUNE_COUNT = 16
 };
 

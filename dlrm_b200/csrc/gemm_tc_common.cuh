@@ -1,7 +1,6 @@
-// Shared pieces of the wgmma GEMM kernels (gemm_tc.cu: one tile per CTA; gemm_chain.cu: persistent
-// tile-dataflow kernel): tile constants, the problem description, PTX wrappers (mbarrier, TMA, wgmma),
-// the wgmma shared-memory descriptor, the consumer main loop, the epilogue and the plan object the C ABI
-// hands out.
+// Pieces of the wgmma GEMM kernel (gemm_tc.cu): tile constants, the problem description, PTX wrappers
+// (mbarrier, TMA, wgmma), the wgmma shared-memory descriptor, the consumer main loop, the epilogue and the
+// plan object the C ABI hands out.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -220,8 +219,7 @@ __device__ __forceinline__ void tc_stage_acc(const float (&d)[BN / 2], float* ac
   }
 }
 
-// Staged tile (128 rows x bn columns) -> global memory, shared by the per-layer kernel (gemm_tc.cu) and the
-// persistent chain kernel (gemm_chain.cu).
+// Staged tile (128 rows x bn columns) -> global memory.
 //
 // Storing straight from the row-per-lane layout would make each warp-wide 16-byte store hit 32 different rows
 // (32 half-written sectors per instruction).  Instead every 32 x 32 chunk is transposed through a per-warp
@@ -233,13 +231,7 @@ constexpr int TC_EPI_ROW_F32 = 20;                 // floats per staged fp32 hal
 constexpr int TC_EPI_ROW_BF16 = 40;                // bf16 per staged bf16 row (32 + 8 pad)
 constexpr int TC_EPI_WARP_BYTES = 32 * TC_EPI_ROW_BF16 * 2;  // 2560 B per epilogue warp (fp32: two 16-column passes)
 constexpr int TC_EPI_BYTES = TC_EPI_WARPS * TC_EPI_WARP_BYTES;
-// persistent chain kernel: dynamic shared memory besides the operand ring (its producer streams the next task's
-// operands while the epilogue runs, so the accumulator needs a region of its own):
-// barriers + task ring | accumulator | per-warp staging | align
-__host__ __device__ constexpr size_t tc_extra_smem(int bn, int head) {
-  return (size_t)head + tc_acc_bytes(bn) + TC_EPI_BYTES + 1024;
-}
-// per-layer kernel: the accumulator is staged in the operand ring, idle once the last wgmma has retired
+// the accumulator is staged in the operand ring, idle once the last wgmma has retired
 __host__ __device__ constexpr size_t tc_ring_bytes(size_t ring, int bn) {
   return ring > (size_t)tc_acc_bytes(bn) ? ring : (size_t)tc_acc_bytes(bn);
 }
@@ -273,9 +265,9 @@ __device__ __forceinline__ void tc_epi_store_bf16(const __nv_bfloat16 (&mine)[32
 // warps per 32-row block split the chunks of a tile between them).
 __device__ __forceinline__ void tc_epilogue_tile(const TcArgs& g, int bn, int m0, int n0, int bz, const float* acc,
                                                  int quad, int lane, uint8_t* stage_warp, int c0, int cstep) {
-  // Every field is copied into a register ONCE: `g` lives in kernel-parameter space (indexed at run time in the
-  // chain kernel) and the mbarrier asm statements clobber memory, so reading g.act or g.bias inside the
-  // element loops costs a constant-bank load + a branch PER ELEMENT.
+  // Every field is copied into a register ONCE: `g` lives in kernel-parameter space and the mbarrier asm
+  // statements clobber memory, so reading g.act or g.bias inside the element loops costs a constant-bank load +
+  // a branch PER ELEMENT.
   const long long M = g.M, N = g.N;
   const int act = g.act, mask_act = g.mask_act;
   const __nv_bfloat16* const mask_hi = g.mask_hi;

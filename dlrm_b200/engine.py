@@ -241,19 +241,9 @@ class Engine:
         self.remote_sample0 = 0      # first global sample of THIS rank (its bags inside the global index streams)
         # side streams: the gather runs beside the bottom MLP, the weight-gradient GEMMs and the
         # embedding update beside the dgrad chain (independent work; parallel branches in the graph)
-        self.multi_stream = True
-        # DLRM_CHAIN=1: every MLP chain (forward layers; dgrad chain + weight gradients) as ONE persistent
-        # tile-dataflow launch (csrc/gemm_chain.cu) instead of one launch per layer.  Bit-identical results
-        # (tests/test_gpu_chain.py).  Opt-in: a CTA that claimed a task whose producer tiles are not done blocks
-        # instead of taking ready work, and the persistent grid shares the SMs with the gather / update kernels of
-        # the embedding stream, so per-layer launches (+ programmatic dependent launch) stay the default.
-        self.use_chain = os.environ.get("DLRM_CHAIN", "0") == "1"
-        self.tc_tile_n = {}          # optional (kind, which, i) -> tile_n override for the wgmma plans
-        self.tc_smem_kb = (0, 0)    # (forward, backward) operand-ring budget of the wgmma GEMM plans, KB; 0 = deepest
         self.s_emb = torch.cuda.Stream(device=self.device)
         self.s_wg = torch.cuda.Stream(device=self.device)
         self.s_small = torch.cuda.Stream(device=self.device)
-        self._gather_events = None   # optional (start, end) CUDA events recorded around the gather
         self._alloc_activations(int(max_batch))
 
     # ------------------------------------------------------------------ buffers
@@ -666,13 +656,8 @@ class Engine:
         outs, lds = self._bot_outs(B)
         self.mlp_forward("bot", X, X.stride(0), B, outs, lds)
         if self.T:
-            ev = self._gather_events
-            if ev is not None:
-                ev[0].record()
             self.emb_forward(sp, link=link)
             self.reduce_partials(B)
-            if ev is not None:
-                ev[1].record()
         if self.op == "dot":
             _lib.check(self.lib.dlrm_b200_interact_fwd(self.Tbuf.data_ptr(), FD, self.Rbuf.data_ptr(),
                                                        self.ldr, B, self.F, self.D, int(self.itself),
@@ -751,7 +736,7 @@ class Engine:
         small = [k for k in range(self.T) if self.is_small(k)]
         # The tiny-table kernels (few, long-running CTAs) go FIRST, on their own stream: they take their SM slots and the
         # grid-stride list-path update fills the rest of the machine beside them (different tables, no ordering needed).
-        side = bool(small) and bool(big) and self.multi_stream and os.environ.get("DLRM_SMALL_SIDE", "1") != "0"
+        side = bool(small) and bool(big) and os.environ.get("DLRM_SMALL_SIDE", "1") != "0"
         if side:
             self._fork(self.s_small)
         with (torch.cuda.stream(self.s_small) if side else contextlib.nullcontext()):
@@ -889,8 +874,7 @@ class Engine:
     def sync_update(self):
         """Make the current stream wait for an embedding update left running by
         train_step(join_update=False)."""
-        if self.multi_stream:
-            self._join(self.s_emb)
+        self._join(self.s_emb)
 
     # ---- entry points used by the DLRM_Net facade (dlrm_b200/dlrm_net.py)
     def backward_from_output_grad(self, X: torch.Tensor, sp: SparseInput, gp: torch.Tensor):
@@ -960,7 +944,7 @@ class Engine:
         must then use a different batch buffer for the next step and call `sync_update()` before
         reading the tables from another stream."""
         self.ensure_optimizer_state(optimizer)
-        self._join_update = bool(join_update) or not self.tc or not self.multi_stream
+        self._join_update = bool(join_update) or not self.tc
         self.forward(X, sp, link=not link_done, skip_head=True)
         self.opt_step += 1
         clr = lr / (1.0 + (self.opt_step - 1.0) * lr_decay) if optimizer in _LR_DECAY else lr
@@ -1093,20 +1077,6 @@ class Engine:
                 Ws.append((torch.zeros((N, Kp), dtype=bf, device=dev), torch.zeros((N, Kp), dtype=bf, device=dev), Kp))
             self.tc_in[which], self.tc_gz[which], self.tc_W[which] = ins, gzs, Ws
         FD = self.F * self.D
-        # operand-ring budget per GEMM CTA (KB; 0 = library default 200, the deepest ring).  A smaller ring only
-        # shortens the pipeline: a wgmma CTA (384 threads, ~160 registers) leaves no room for a second one on the SM.
-        fwd_kb = int(os.environ.get("DLRM_TC_FWD_SMEM_KB", self.tc_smem_kb[0]))
-        bwd_kb = int(os.environ.get("DLRM_TC_BWD_SMEM_KB", self.tc_smem_kb[1]))
-
-        def GP(_kb, **kw):
-            if "tile_n" not in kw:
-                kw["tile_n"] = int(os.environ.get("DLRM_CHAIN_TILE_N", "0"))   # experiment knob; 0 = auto
-            _lib.set_tunable("gemm_smem_kb", _kb)
-            try:
-                return _lib.GemmTcPlan(**kw)
-            finally:
-                _lib.set_tunable("gemm_smem_kb", 0)
-
         for which in ("bot", "top"):
             ln = self.ln_bot if which == "bot" else self.ln_top
             ntc = self.ntc[which]
@@ -1129,12 +1099,12 @@ class Engine:
                     kw.update(out_f32=self.Tbuf.data_ptr(), ld_f32=FD)
                 elif which == "top" and (i == ntc - 1):
                     kw.update(out_f32=self.top_act[i].data_ptr(), ld_f32=self.top_act[i].shape[1])
-                self.tc_plans["fwd"][(which, i)] = GP(fwd_kb, **kw)
+                self.tc_plans["fwd"][(which, i)] = _lib.GemmTcPlan(**kw)
                 # ---- wgrad: [dW | db] = gz^T [X | 1]   (both operands read MN-major, split-K slabs)
                 oW = self._dense_off[(which, i, "W")]
                 ob = self._dense_off[(which, i, "b")]
-                self.tc_plans["wgrad"][(which, i)] = GP(
-                    bwd_kb, A_hi=gh.data_ptr(), A_lo=gl.data_ptr(), lda=Np, a_mn_major=1,
+                self.tc_plans["wgrad"][(which, i)] = _lib.GemmTcPlan(
+                    A_hi=gh.data_ptr(), A_lo=gl.data_ptr(), lda=Np, a_mn_major=1,
                     B_hi=ih.data_ptr(), B_lo=il.data_ptr(), ldb=Kp, b_mn_major=1,
                     M=N, N=K + 1, K=B, mode_x3=x3, split_k=want_splits[(which, i)],
                     out_f32=self.dense_grad.data_ptr() + oW * 4, ld_f32=K, slab_stride=P,
@@ -1144,20 +1114,18 @@ class Engine:
                 # ---- dgrad: gz_prev = (gz W) * act'(input activation)
                 if i > 0:
                     ph, pl, Np_prev = self.tc_gz[which][i - 1]
-                    self.tc_plans["dgrad"][(which, i)] = GP(
-                        bwd_kb, A_hi=gh.data_ptr(), A_lo=gl.data_ptr(), lda=Np, a_mn_major=0,
+                    self.tc_plans["dgrad"][(which, i)] = _lib.GemmTcPlan(
+                        A_hi=gh.data_ptr(), A_lo=gl.data_ptr(), lda=Np, a_mn_major=0,
                         B_hi=wh.data_ptr(), B_lo=wl.data_ptr(), ldb=Kp, b_mn_major=1,
                         M=B, N=K, K=N, mode_x3=x3, split_k=1,
                         mask_act=self._act(which, i - 1), mask_hi=ih.data_ptr(), mask_lo=il.data_ptr(), ldmask=Kp,
                         out_hi=ph.data_ptr(), out_lo=pl.data_ptr(), ld_out=Np_prev)
                 elif which == "top" and self.op == "dot":
-                    self.tc_plans["dgrad"][(which, 0)] = GP(
-                        bwd_kb, A_hi=gh.data_ptr(), A_lo=gl.data_ptr(), lda=Np, a_mn_major=0,
+                    self.tc_plans["dgrad"][(which, 0)] = _lib.GemmTcPlan(
+                        A_hi=gh.data_ptr(), A_lo=gl.data_ptr(), lda=Np, a_mn_major=0,
                         B_hi=wh.data_ptr(), B_lo=wl.data_ptr(), ldb=Kp, b_mn_major=1,
                         M=B, N=K, K=N, mode_x3=x3, split_k=1,
                         out_f32=self.dR.data_ptr(), ld_f32=self.ldr)
-        if self.use_chain:
-            self._build_chains()
         self._pack_dirty = True
 
     def _split(self, x: torch.Tensor, ldx: int, M: int, N: int, hl):
@@ -1210,13 +1178,9 @@ class Engine:
         ln = self.ln_bot if which == "bot" else self.ln_top
         s = _stream()
         ntc = self.ntc[which]
-        if self.use_chain and ntc:
-            self.tc_chains[("fwd", which)].run(s)
+        for i in range(ntc):
+            self.tc_plans["fwd"][(which, i)].run(s)
             self.n_launch += 1
-        else:
-            for i in range(ntc):
-                self.tc_plans["fwd"][(which, i)].run(s)
-                self.n_launch += 1
         nl = len(ln) - 1
         if which == "top" and self.has_head:
             nl -= 1
@@ -1238,9 +1202,9 @@ class Engine:
         if self.ntc["bot"] == 0 or self.ntc["top"] == 0 or self.op != "dot":
             raise RuntimeError("gemm='tc' needs op='dot' and MLP layers of width >= 16; use gemm='simt'")
         FD = self.F * self.D
-        ms = self.multi_stream and (self.T > 0 or self.gather_fn is not None)
+        gather = self.T > 0 or self.gather_fn is not None
         self._mark("begin")
-        if ms:   # gather (+ link) beside the bottom MLP
+        if gather:   # gather (+ link) beside the bottom MLP
             self._fork(self.s_emb)
             with torch.cuda.stream(self.s_emb):
                 if self.gather_fn is not None:
@@ -1253,19 +1217,9 @@ class Engine:
         self._split(X, X.stride(0), B, self.ln_bot[0], self.tc_in["bot"][0])
         self._tc_mlp_forward("bot", B)
         self._mark("bot_fwd")
-        if ms:
+        if gather:
             self._join(self.s_emb)
             self._mark("join_gather")
-        elif self.gather_fn is not None:
-            self.gather_fn(sp, link)
-        elif self.T:
-            ev = self._gather_events
-            if ev is not None:
-                ev[0].record()
-            self.emb_forward(sp, link=link)
-            self.reduce_partials(B)
-            if ev is not None:
-                ev[1].record()
         rh, rl, ldrb = self.tc_in["top"][0]
         if self.D % 4 == 0:
             # R goes straight to the (hi, lo) operand pair of the first top-MLP GEMM
@@ -1287,57 +1241,17 @@ class Engine:
         return p
 
     def _tc_mlp_backward(self, which: str, B: int):
-        """gz of the last tensor-core layer is ready on the current stream.  Chain mode: dgrads and weight
-        gradients of the whole MLP are ONE persistent launch.  Per-layer mode: dgrads stay on this stream
-        (the critical chain); every wgrad only feeds the final dense update and goes to the side stream."""
-        if self.use_chain:
-            self.tc_chains[("bwd", which)].run(_stream())
-            self.n_launch += 1
-            return
+        """gz of the last tensor-core layer is ready on the current stream.  The dgrads stay on this stream (the
+        critical chain); every wgrad only feeds the final dense update and goes to the side stream."""
         for i in reversed(range(self.ntc[which])):
-            if self.multi_stream:
-                self._fork(self.s_wg)   # gz_i was produced by the previous launch on this stream
-                with torch.cuda.stream(self.s_wg):
-                    self.tc_plans["wgrad"][(which, i)].run(_stream())
-            else:
+            self._fork(self.s_wg)   # gz_i was produced by the previous launch on this stream
+            with torch.cuda.stream(self.s_wg):
                 self.tc_plans["wgrad"][(which, i)].run(_stream())
             self.n_launch += 1
             pl = self.tc_plans["dgrad"].get((which, i))
             if pl is not None:
                 pl.run(_stream())
                 self.n_launch += 1
-
-    def _build_chains(self):
-        """Group the per-layer plans into persistent launches.  forward: layer i reads layer i-1's rows.
-        backward (order = claim order): dgrad_i (critical chain, reads dgrad_{i+1}'s rows), then wgrad_i
-        (reads gz_i = dgrad_{i+1}'s output over its k range = batch rows)."""
-        self.tc_chains, self._chain_ctr = {}, {}
-        for which in ("bot", "top"):
-            ntc = self.ntc[which]
-            if ntc == 0:
-                continue
-            plans = [self.tc_plans["fwd"][(which, i)] for i in range(ntc)]
-            self._make_chain(("fwd", which), plans, [-1] + list(range(ntc - 1)), [0] * ntc)
-            # dgrad chain first (one m-tile-major group), then every weight gradient
-            plans, dep, onk = [], [], []
-            producer = {}               # layer i -> position of the dgrad that produced gz_i (absent: earlier kernel)
-            prev = -1
-            for i in reversed(range(ntc)):
-                producer[i] = prev
-                pl = self.tc_plans["dgrad"].get((which, i))
-                if pl is not None:
-                    plans.append(pl); dep.append(prev); onk.append(0)
-                    prev = len(plans) - 1
-                else:
-                    prev = -1
-            for i in reversed(range(ntc)):
-                plans.append(self.tc_plans["wgrad"][(which, i)]); dep.append(producer[i]); onk.append(1)
-            self._make_chain(("bwd", which), plans, dep, onk)
-
-    def _make_chain(self, key, plans, dep, onk):
-        ctr = torch.zeros(_lib.GemmChain.counters_needed(plans), dtype=torch.int32, device=self.device)
-        self._chain_ctr[key] = ctr
-        self.tc_chains[key] = _lib.GemmChain(plans, dep, onk, ctr)
 
     def _tc_backward(self, X: torch.Tensor, sp: SparseInput, target: torch.Tensor, update=None):
         B = X.shape[0]
@@ -1391,23 +1305,17 @@ class Engine:
             opt, clr = update
             upd = (lambda: self.update_fn(sp, opt, clr)) if self.update_fn is not None else \
                 (lambda: self.emb_update(sp, optimizer=opt, lr=clr))
-            if self.multi_stream:
-                self._fork(self.s_emb)
-                with torch.cuda.stream(self.s_emb):
-                    upd()
-                    self._mark("emb:update")
-            else:
+            self._fork(self.s_emb)
+            with torch.cuda.stream(self.s_emb):
                 upd()
                 self._mark("emb:update")
         self._tc_mlp_backward("bot", B)
         self._mark("bot_bwd_dgrad")
-        if self.multi_stream:
-            if not self.use_chain:
-                self._join(self.s_wg)
-                self._mark("join_wgrads")
-            if update is not None and has_emb and getattr(self, "_join_update", True):
-                self._join(self.s_emb)
-                self._mark("join_update")
+        self._join(self.s_wg)
+        self._mark("join_wgrads")
+        if update is not None and has_emb and getattr(self, "_join_update", True):
+            self._join(self.s_emb)
+            self._mark("join_update")
 
 
 def _refuse_graphed_f16(eng: "Engine"):

@@ -400,28 +400,6 @@ int dlrm_b200_gemm_tc_plan_info(void* plan, int* tile_n, int* stages, int* split
 int dlrm_b200_gemm_tc_run(void* plan, void* stream);
 int dlrm_b200_gemm_tc_plan_destroy(void* plan);
 
-/* A whole MLP chain in ONE persistent launch (apply_mlp: `layers(x)`, dlrm_s_pytorch.py:399-405, and its
- * autograd: the dgrad chain with every weight-gradient GEMM beside it, :1613).  The plans' output tiles form
- * one topologically ordered task list (plan order; inside a plan: n tile, m tile, k split); one CTA per SM
- * claims tasks from a device-side queue and runs TMA -> wgmma -> epilogue; the TMA producer already
- * streams the next tile's operands while the consumers run the epilogue of this one.  dep[i] >= 0 names the plan
- * that produces plan i's A operand inside this launch: a task waits until every 128-row block of that
- * producer covering its A rows (dep_on_k[i] = 0: the task's own m tile; = 1: the task's k range, i.e. a
- * weight-gradient GEMM reducing over the batch) is complete (per-block counters, release/acquire at GPU
- * scope + async-proxy fence before the TMA reads).  Results are bit-identical to running the plans one by
- * one.  counters: caller-owned, zero-initialised int32[counters_len], counters_len >= 2 + sum of the
- * plans' m tiles; the kernel leaves it zeroed.  Plans must outlive the chain. */
-int dlrm_b200_gemm_chain_create(void* const* plans /*[host][n]*/, const int* dep /*[host][n]*/,
-                                const int* dep_on_k /*[host][n]*/, int n, int32_t* counters,
-                                int64_t counters_len, void** chain);
-int dlrm_b200_gemm_chain_info(void* chain, int* tasks, int* ctas, int* stages, int* smem_bytes);
-/* Optional per-task timeline for tools/chain_timeline.py: trace = device uint64[8 * tasks] (globaltimer ns: task
- * claimed, dependencies ready, last TMA issued, first operands landed, last MMA issued, accumulator ready,
- * epilogue + signal done; word 7 = SM id), or NULL to switch it off (default). */
-int dlrm_b200_gemm_chain_set_trace(void* chain, uint64_t* trace);
-int dlrm_b200_gemm_chain_run(void* chain, void* stream);
-int dlrm_b200_gemm_chain_destroy(void* chain);
-
 /* fp32 [M,N] (row stride ldx) -> (hi, lo) bf16 [M, ld_out]; lo may be NULL */
 int dlrm_b200_split_bf16(const float* X, int64_t ldx, int64_t M, int64_t N, void* hi, void* lo,
                          int64_t ld_out, void* stream);
