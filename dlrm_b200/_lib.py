@@ -43,6 +43,18 @@ class EmbDedup(C.Structure):
     _fields_ = [("filter", C.c_void_p), ("log2_size", C.c_int32), ("flags", C.c_void_p), ("suspects", C.c_void_p)]
 
 
+class HostTable(C.Structure):
+    _fields_ = [("weight", C.c_void_p), ("momentum", C.c_void_p), ("acc_ew", C.c_void_p), ("indices", C.c_void_p),
+                ("offsets", C.c_void_p), ("nnz", C.c_int64), ("rows", C.c_int64), ("pos_base", C.c_int64),
+                ("map", C.c_void_p)]
+
+
+class HostStage(C.Structure):
+    _fields_ = [("weight", C.c_void_p), ("momentum", C.c_void_p), ("head", C.c_void_p), ("acc_ew", C.c_void_p),
+                ("slot_idx", C.c_void_p), ("list", C.c_void_p), ("key", C.c_void_p), ("count", C.c_void_p),
+                ("capacity", C.c_int64), ("ld", C.c_int64), ("head_col", C.c_int64)]
+
+
 class GemmTcDesc(C.Structure):
     _fields_ = [("A_hi", C.c_void_p), ("A_lo", C.c_void_p), ("lda", C.c_int64), ("a_mn_major", C.c_int),
                 ("B_hi", C.c_void_p), ("B_lo", C.c_void_p), ("ldb", C.c_int64), ("b_mn_major", C.c_int),
@@ -83,6 +95,8 @@ SYMBOLS = [
     "dlrm_b200_emb_bwd_small_scratch_bytes", "dlrm_b200_emb_bwd_small_update", "dlrm_b200_emb_reduce_partials",
     "dlrm_b200_block_copy", "dlrm_b200_gen_multihot", "dlrm_b200_set_tunable", "dlrm_b200_emb_bag_fwd_remote", "dlrm_b200_split_bf16", "dlrm_b200_dense_update_pack",
     "dlrm_b200_decode_records", "dlrm_b200_gather_records", "dlrm_b200_ingest_records",
+    "dlrm_b200_host_stage_in", "dlrm_b200_host_write_back", "dlrm_b200_host_release", "dlrm_b200_host_register",
+    "dlrm_b200_host_unregister",
 ]
 
 
@@ -142,6 +156,11 @@ def _declare(lib):
     lib.dlrm_b200_decode_records.argtypes = [vp, i64, i32, i32, i64, vp, vp, vp, vp, vp]
     lib.dlrm_b200_gather_records.argtypes = [vp, vp, vp, vp, i64, i32, i32, i64, vp, vp, vp, vp, vp]
     lib.dlrm_b200_ingest_records.argtypes = [vp, i32, vp, i32, vp, i32, i64, i32, i32, vp, vp, vp, i64, i64, vp, vp]
+    lib.dlrm_b200_host_stage_in.argtypes = [C.POINTER(HostTable), i32, C.POINTER(HostStage), i32, i64, i32, i32, vp]
+    lib.dlrm_b200_host_write_back.argtypes = [C.POINTER(HostTable), i32, C.POINTER(HostStage), i32, vp]
+    lib.dlrm_b200_host_release.argtypes = [C.POINTER(HostTable), i32, C.POINTER(HostStage), i32, vp]
+    lib.dlrm_b200_host_register.argtypes = [vp, i64]
+    lib.dlrm_b200_host_unregister.argtypes = [vp]
     for name in SYMBOLS:
         fn = getattr(lib, name)
         if name in ("dlrm_b200_head_scratch_bytes", "dlrm_b200_emb_bwd_small_scratch_bytes"):

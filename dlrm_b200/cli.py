@@ -99,6 +99,9 @@ def build_parser():
     p.add_argument("--gemm", type=str, default="tc", choices=["tc", "tc_bf16", "simt"])
     # dlrm_b200 addition: storage type of the embedding tables (fp16: stochastically rounded row updates)
     p.add_argument("--emb-dtype", type=str, default="fp32", choices=["fp32", "fp16"])
+    # dlrm_b200 addition: tables kept in pinned host memory, their touched rows staged through HBM every step
+    # ("" none, "auto": the largest tables until the rest fits in device memory, or dash-separated table ids)
+    p.add_argument("--emb-host-tables", type=str, default="")
     return p
 
 
@@ -157,6 +160,18 @@ class LRPolicy:
             lr = self.last if self.steps > 0 else self.base
         for g, v in zip(self.opt.param_groups, lr):
             g["lr"] = v
+
+
+def _auto_adagrad(ln_emb, m_spa, device):
+    """--emb-host-tables=auto with --optimizer=adagrad: every row also carries its element-wise accumulators."""
+    from . import host_tables as ht
+    from .dlrm_net import DLRM_Net
+
+    free, _ = torch.cuda.mem_get_info(device)
+    try:
+        return ht.auto_host_tables(ln_emb.tolist(), 8 * int(m_spa) + 8, free, DLRM_Net.host_reserve(m_spa, ln_emb))
+    except ValueError as e:
+        sys.exit("ERROR: " + str(e))
 
 
 def run(argv=None):
@@ -367,13 +382,38 @@ def run(argv=None):
     nbatches_test = len(test_data)
 
     loss_ws = np.fromstring(args.loss_weights, dtype=float, sep="-") if args.loss_function == "wbce" else None
+    host_tables = None
+    if args.emb_host_tables:
+        from . import host_tables as ht
+
+        try:
+            host_tables = ht.parse(args.emb_host_tables, ln_emb.size)
+        except ValueError as e:
+            sys.exit("ERROR: " + str(e))
+        if args.emb_dtype == "fp16":
+            sys.exit("ERROR: --emb-host-tables needs --emb-dtype=fp32 (the stochastic rounding of fp16 tables is keyed "
+                     "by the row index the update kernel sees)")
+        if world > 1:
+            sys.exit("ERROR: --emb-host-tables is not supported on sharded runs (torchrun)")
+        if args.weighted_pooling is not None:
+            sys.exit("ERROR: --emb-host-tables does not support weighted pooling (row weights are indexed by table "
+                     "row)")
+        if host_tables != "auto":
+            tiny = [k for k in host_tables if int(ln_emb[k]) <= 256]
+            if tiny:
+                sys.exit("ERROR: --emb-host-tables: table %d has %d rows: tiny tables (<= 256 rows) take the dense "
+                         "two-pass update, which indexes the whole table on the device"
+                         % (tiny[0], int(ln_emb[tiny[0]])))
+        if host_tables == "auto" and args.optimizer == "adagrad":
+            host_tables = _auto_adagrad(ln_emb, m_spa, device)
     dlrm = DLRM_Net(m_spa, ln_emb, ln_bot, ln_top, arch_interaction_op=args.arch_interaction_op,
                     arch_interaction_itself=args.arch_interaction_itself, sigmoid_bot=-1,
                     sigmoid_top=ln_top.size - 2, sync_dense_params=args.sync_dense_params,
                     loss_threshold=args.loss_threshold, ndevices=-1, weighted_pooling=args.weighted_pooling,
                     loss_function=args.loss_function, device=device, gemm=args.gemm,
                     max_batch=args.mini_batch_size, loss_weights=loss_ws,
-                    emb_dtype=torch.float16 if args.emb_dtype == "fp16" else torch.float32)
+                    emb_dtype=torch.float16 if args.emb_dtype == "fp16" else torch.float32,
+                    emb_host_tables=host_tables or None)
     optimizer = lr_scheduler = None
     if not args.inference_only:
         opts = {"sgd": fused.SGD, "rwsadagrad": fused.RWSAdagrad, "adagrad": fused.Adagrad}   # :1342-1346
@@ -412,7 +452,9 @@ def run(argv=None):
     total_time = total_loss = total_iter = total_samp = 0
     if args.load_model:                                      # dlrm_s_pytorch.py:1399-1456
         print("Loading saved model {}".format(args.load_model))
-        ld = torch.load(args.load_model, map_location=device, weights_only=False)
+        # host tables: the checkpoint's tables stay in (memory-mapped) host memory; load_state_dict copies them in place
+        ld = (torch.load(args.load_model, map_location="cpu", mmap=True, weights_only=False) if host_tables
+              else torch.load(args.load_model, map_location=device, weights_only=False))
         dlrm.load_state_dict(ld["state_dict"])
         ld_j, ld_k = ld["iter"], ld["epoch"]
         ld_nepochs, ld_nbatches, ld_nbatches_test = ld["nepochs"], ld["nbatches"], ld["nbatches_test"]

@@ -19,7 +19,10 @@ one autograd node whose backward runs the engine's backward kernels.  Embedding 
 `emb_dtype=torch.float16` stores the tables as fp16 (`emb_l[k].weight` is an fp16 strided parameter): lookups widen
 the rows to fp32, the fused optimizers update them in fp32 and store them with stochastic rounding.  `state_dict()`
 then holds fp16 tables; an fp32 checkpoint loads with round-to-nearest, an fp16 one into an fp32 model exactly.
-QR / mixed-dimension embeddings, quantised embeddings and `parallel_forward` are outside the path
+`emb_host_tables="auto" | [k, ...]` keeps those tables in pinned host memory (dlrm_b200/host_tables.py): their
+`emb_l[k].weight` are CPU tensors, so `state_dict()` / `load_state_dict()` and checkpoints are unchanged, and every step
+stages the rows the batch touches through HBM.  "auto" moves the largest tables until the rest fits in free device
+memory.  QR / mixed-dimension embeddings, quantised embeddings and `parallel_forward` are outside the path
 (SURVEY §2) and exit with an error when requested.
 """
 from __future__ import annotations
@@ -92,6 +95,9 @@ class _DLRMForward(torch.autograd.Function):
         net, eng = ctx.net, ctx.net._engine
         eng.backward_from_output_grad(ctx.x, ctx.sp, gp.contiguous())
         grads: List[Optional[torch.Tensor]] = []
+        if net._fused_opt is None and eng.host:
+            raise RuntimeError("dlrm_b200: host embedding tables are trained by the fused optimizers of "
+                               "dlrm_b200.optim (SGD, RWSAdagrad, Adagrad); create one before calling backward()")
         if net._fused_opt is None and eng.f16:
             raise RuntimeError("dlrm_b200: fp16 embedding tables are trained by the fused optimizers of "
                                "dlrm_b200.optim (SGD, RWSAdagrad); create one before calling backward()")
@@ -116,7 +122,7 @@ class DLRM_Net(nn.Module):
                  loss_threshold=0.0, ndevices=-1, qr_flag=False, qr_operation="mult", qr_collisions=0,
                  qr_threshold=200, md_flag=False, md_threshold=200, weighted_pooling=None,
                  loss_function="bce", *, device=None, gemm="tc", max_batch=2048, loss_weights=None,
-                 emb_dtype=torch.float32, round_seed=0):
+                 emb_dtype=torch.float32, round_seed=0, emb_host_tables=None):
         super().__init__()
         self._engine: Optional[Engine] = None
         self._fused_opt = None
@@ -166,6 +172,27 @@ class DLRM_Net(nn.Module):
         self._dist = None
         import torch.distributed as tdist
 
+        host = []
+        if emb_host_tables:
+            if emb_dtype == "fp16":
+                sys.exit("ERROR: host embedding tables need fp32 rows (the stochastic rounding of fp16 tables is keyed "
+                         "by the row index the update kernel sees)")
+            if weighted_pooling is not None:
+                sys.exit("ERROR: host embedding tables do not support weighted pooling (row weights are indexed by "
+                         "table row)")
+            if tdist.is_available() and tdist.is_initialized() and tdist.get_world_size() > 1:
+                sys.exit("ERROR: host embedding tables are not supported on sharded runs")
+            if emb_host_tables == "auto":
+                from .host_tables import auto_host_tables
+
+                free, _ = torch.cuda.mem_get_info(torch.device(device) if device is not None else None)
+                try:
+                    host = auto_host_tables(ln_emb.tolist(), 4 * int(m_spa) + 8, free, self.host_reserve(m_spa, ln_emb))
+                except ValueError as e:
+                    sys.exit("ERROR: " + str(e))
+            else:
+                host = sorted(set(int(k) for k in emb_host_tables))
+
         if tdist.is_available() and tdist.is_initialized() and tdist.get_world_size() > 1:
             # one process per GPU (the reference: ext_dist.my_size > 1, dlrm_s_pytorch.py:352-365): tables are
             # placed over the ranks (dlrm_b200/placement.py), the MLPs replicated; max_batch is the GLOBAL batch
@@ -189,7 +216,7 @@ class DLRM_Net(nn.Module):
                                   sigmoid_bot=sigmoid_bot, sigmoid_top=sigmoid_top, loss=loss_function,
                                   loss_threshold=loss_threshold, loss_ws=loss_ws, device=device,
                                   max_batch=max_batch, gemm=gemm, emb_dtype=emb_dtype, round_seed=round_seed,
-                                  interleave_momentum=None if emb_dtype == "fp16" else False)
+                                  interleave_momentum=None if emb_dtype == "fp16" else False, host_tables=host)
         self._m_spa, self._ln_emb = int(m_spa), ln_emb
         # same construction (and numpy RNG consumption) order as the reference: tables, bottom, top
         if ndevices <= 1:
@@ -211,6 +238,23 @@ class DLRM_Net(nn.Module):
         ref = weakref.ref(self)
         for p in self.parameters():
             p._dlrm_net = ref
+
+    @staticmethod
+    def host_reserve(m_spa, ln_emb) -> int:
+        """Device bytes "auto" keeps free beside the tables: 2 GiB of activations and workspace, plus the largest table
+        once, which a large table's initial draw uses on the device before it is copied to host memory."""
+        big = int(np.sum(ln_emb)) * int(m_spa) > _NUMPY_INIT_MAX
+        return (1 << 31) + (int(np.max(ln_emb)) * int(m_spa) * 4 if big else 0)
+
+    def state_dict(self, *args, **kwargs):
+        if self._engine is not None and self._engine.host:
+            self._engine._host_sync()       # host rows may still be on their way back from the last step
+        return super().state_dict(*args, **kwargs)
+
+    def load_state_dict(self, state_dict, *args, **kwargs):
+        if self._engine is not None and self._engine.host:
+            self._engine._host_sync()
+        return super().load_state_dict(state_dict, *args, **kwargs)
 
     # ------------------------------------------------------------------ construction
     def create_mlp(self, ln, sigmoid_layer):
@@ -272,7 +316,13 @@ class DLRM_Net(nn.Module):
             tab = eng.table(k)
             a = float(np.sqrt(1 / n))
             with torch.no_grad():
-                if big:
+                if big and eng.is_host[k]:
+                    # the draw of a device table (same sizes and strides), then copied to host memory
+                    tmp = torch.empty(tab.shape, dtype=torch.float32, device=eng.device)
+                    _uniform_(tmp, a, gen)
+                    tab.copy_(tmp)
+                    del tmp
+                elif big:
                     _uniform_(tab, a, gen)
                 else:  # bit-identical to the reference for the same numpy seed (dlrm_s_pytorch.py:280-284)
                     W = np.random.uniform(low=-a, high=a, size=(n, int(m))).astype(np.float32)

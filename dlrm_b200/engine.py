@@ -100,7 +100,7 @@ class Engine:
                  loss: str = "bce", loss_threshold: float = 0.0, loss_ws=None, device="cuda:0",
                  max_batch: int = 2048, gemm: str = "simt", n_features: Optional[int] = None,
                  interleave_momentum: Optional[bool] = None, shards=None, split_slots=None, small_rows_max: int = 256,
-                 emb_dtype: str = "fp32", round_seed: int = 0):
+                 emb_dtype: str = "fp32", round_seed: int = 0, host_tables: Sequence[int] = ()):
         if not torch.cuda.is_available():
             raise RuntimeError("dlrm_b200.Engine needs a CUDA device (H100, sm_90a); there is no CPU path")
         self.device = torch.device(device)
@@ -176,6 +176,17 @@ class Engine:
         rows = np.asarray(self.ln_emb, dtype=np.int64)
         self.row_base = np.concatenate([[0], np.cumsum(rows)]).astype(np.int64)
         self.total_rows = int(self.row_base[-1])
+        # Host tables (dlrm_b200/host_tables.py): their rows live in pinned host memory and the rows of each batch are
+        # staged through HBM.  Every table keeps its rows in ONE arena, device or host; _abase[k] is its first row
+        # there (== row_base[k] when no table is on the host).
+        self.host = sorted(set(int(k) for k in host_tables))
+        self.is_host = [k in self.host for k in range(self.T)]
+        self._check_host_tables(interleave_momentum)
+        self._abase, nb = [], [0, 0]
+        for k, n in enumerate(self.ln_emb):
+            self._abase.append(nb[self.is_host[k]])
+            nb[self.is_host[k]] += n
+        self.dev_rows, self.host_rows = nb
         # Row layout.  interleave (default when D % 4 == 0): [D weights | Adagrad accumulator | list head (int32) |
         # 2 pad], row stride D + 4 floats -- the two per-row words of the backward live in the row's own DRAM page.
         # The update kernel is bound by the RATE of random DRAM accesses, not by bytes: a 4-byte head[] read costs
@@ -191,8 +202,9 @@ class Engine:
         self.ldw = self.D + self.row_pad if self.interleave else self.D        # row stride in stored elements
         if self.f16:
             self.ldw = fp16_row_stride(self.D)      # D + 8 halves at D % 8 == 0: 272 bytes at D = 128
-        self.tables = torch.zeros((self.total_rows, self.ldw), dtype=self.wdtype, device=dev)
-        self._head_sep = None if self.interleave else torch.zeros(self.total_rows, dtype=torch.int32, device=dev)
+        self.tables = torch.zeros((self.dev_rows, self.ldw), dtype=self.wdtype, device=dev)
+        self._head_sep = None if self.interleave else torch.zeros(self.dev_rows, dtype=torch.int32, device=dev)
+        self._host_init()
         self._momentum_sep: Optional[torch.Tensor] = None
         self.acc_ew: Optional[torch.Tensor] = None       # element-wise Adagrad accumulators [total_rows, D]
         self.row_weights: Optional[torch.Tensor] = None  # weighted pooling v_W_l, arena [total_rows]
@@ -377,9 +389,169 @@ class Engine:
             self.dedup = d
         self._filtered = False
 
+    # ------------------------------------------------------------------ host tables (csrc/host_tables.cu)
+    def _check_host_tables(self, interleave_momentum):
+        if not self.host:
+            return
+        bad = [k for k in self.host if not 0 <= k < self.T]
+        if bad:
+            raise ValueError("host_tables: table %d does not exist (%d tables)" % (bad[0], self.T))
+        if self.f16:
+            raise ValueError("host tables need fp32 rows: the stochastic rounding of fp16 tables is keyed by the row "
+                             "index the update kernel sees, which is a staging slot for a host table")
+        if any(int(s["nparts"]) != 1 or int(s["row_lo"]) != 0 or int(s["table"]) != k
+               for k, s in enumerate(self.shards)):
+            raise ValueError("host tables are not supported on sharded runs")
+        tiny = [k for k in self.host if self.is_small(k)]
+        if tiny:
+            raise ValueError("host_tables: table %d has %d rows (<= small_rows_max=%d): tiny tables take the dense "
+                             "two-pass update, which indexes the whole table on the device"
+                             % (tiny[0], self.ln_emb[tiny[0]], self.small_rows_max))
+
+    def _pinned_zeros(self, shape) -> torch.Tensor:
+        """Zeros in page-locked host memory mapped at the same device address (cudaHostRegister on a plain CPU tensor:
+        torch's pinned allocator would round every block up to a power of two)."""
+        t = torch.zeros(shape, dtype=torch.float32)
+        nbytes = t.numel() * 4
+        if nbytes:
+            _lib.check(self.lib.dlrm_b200_host_register(t.data_ptr(), nbytes), "host_register")
+            self._pinned.append(t)
+            self.pinned_bytes += nbytes
+        return t
+
+    def _host_init(self):
+        self._pinned: List[torch.Tensor] = []
+        self.pinned_bytes = 0
+        self.tables_h = self._momentum_sep_h = self.acc_ew_h = None
+        self._staged = None             # SparseInput whose host-table rows are in the staging arena
+        self._staged_by_link = False
+        self.stage_cap = 0
+        if not self.host:
+            return
+        import weakref
+
+        self.tables_h = self._pinned_zeros((self.host_rows, self.ldw))
+        self._map_base = {}
+        n = 0
+        for k in self.host:
+            self._map_base[k] = n
+            n += self.ln_emb[k]
+        self.slot_map = torch.zeros(n, dtype=torch.int32, device=self.device)   # slot + 1 of a staged row, else 0
+        self.stage_count = torch.zeros(1, dtype=torch.int32, device=self.device)
+        self._slot_idx = {}
+        weakref.finalize(self, _unpin, self.lib, self._pinned)
+
+    def _host_sync(self):
+        """Host reads and writes of host rows wait for every staging copy the engine has enqueued."""
+        torch.cuda.synchronize(self.device)
+
+    def _ensure_stage(self, cap: int, idx_bytes: int):
+        """Staging arena for `cap` positions (one slot per position of the batch)."""
+        dev = self.device
+        if cap > self.stage_cap:
+            self.stage_cap = cap
+            self.stage_w = torch.zeros((cap, self.ldw), dtype=torch.float32, device=dev)
+            self.stage_head = None if self.interleave else torch.zeros(cap, dtype=torch.int32, device=dev)
+            self.stage_list = torch.zeros(cap, dtype=torch.int32, device=dev)
+            self.stage_key = torch.zeros(cap, dtype=torch.int64, device=dev)
+            self.stage_mom = self.stage_acc = None
+            self._slot_idx = {}
+        if self._momentum_sep_h is not None and self.stage_mom is None:
+            self.stage_mom = torch.zeros(self.stage_cap, dtype=torch.float32, device=dev)
+        if self.acc_ew_h is not None and self.stage_acc is None:
+            self.stage_acc = torch.zeros((self.stage_cap, self.D), dtype=torch.float32, device=dev)
+        if idx_bytes not in self._slot_idx:
+            dt = torch.int64 if idx_bytes == 8 else torch.int32
+            self._slot_idx[idx_bytes] = torch.zeros(self.stage_cap, dtype=dt, device=dev)
+
+    def _pos_base(self, sp: SparseInput, k: int) -> int:
+        """First global position of table k: packed batches' offsets are global already; reference-format tables
+        are numbered back to back (the pair_base of the update)."""
+        return 0 if sp.include_last else sum(int(sp.indices[j].numel()) for j in range(k))
+
+    def _slot_ptr(self, sp: SparseInput, k: int) -> int:
+        return self._slot_idx[sp.idx_bytes].data_ptr() + self._pos_base(sp, k) * sp.idx_bytes
+
+    def _host_desc(self, sp: SparseInput):
+        arr = (_lib.HostTable * len(self.host))()
+        for n, k in enumerate(self.host):
+            d = arr[n]
+            d.weight = self.tables_h.data_ptr() + self._abase[k] * self.ldw * 4
+            if self._momentum_sep_h is not None:
+                d.momentum = self._momentum_sep_h.data_ptr() + self._abase[k] * 4
+            if self.acc_ew_h is not None:
+                d.acc_ew = self.acc_ew_h.data_ptr() + self._abase[k] * self.D * 4
+            d.rows = self.ln_emb[k]
+            d.map = self.slot_map.data_ptr() + self._map_base[k] * 4
+            d.indices = sp.indices[k].data_ptr() if sp.indices[k].numel() else 0
+            d.offsets = sp.offsets[k].data_ptr()
+            d.nnz = sp.indices[k].numel()
+            d.pos_base = self._pos_base(sp, k)
+        st = _lib.HostStage()
+        st.weight, st.list, st.key = self.stage_w.data_ptr(), self.stage_list.data_ptr(), self.stage_key.data_ptr()
+        st.momentum = _ptr(self.stage_mom) if self._momentum_sep_h is not None else None
+        st.acc_ew = _ptr(self.stage_acc) if self.acc_ew_h is not None else None
+        st.head = _ptr(self.stage_head)
+        st.count, st.capacity, st.ld = self.stage_count.data_ptr(), self.stage_cap, self.ldw
+        st.head_col = self._meta_col + 1 if self.interleave else -1
+        st.slot_idx = self._slot_idx[sp.idx_bytes].data_ptr()
+        return arr, st
+
+    def _stage_in(self, sp: SparseInput, by_link: bool = False):
+        """Stage the rows of this batch's host-table occurrences (current stream).  A staging left by a step that did
+        not finish is written back first (its rows are unchanged or updated; either way they go home)."""
+        if self.use_filter:
+            raise ValueError("host tables do not support the duplicate filter (use_filter)")
+        if self.row_weights is not None:
+            raise ValueError("host tables do not support weighted pooling: row_weights is indexed by the table row")
+        if self._staged is not None:
+            self._stage_out(True)
+        if sp.include_last and len({sp.indices[k].data_ptr() for k in self.host}) > 1:
+            raise ValueError("host tables: a packed batch must hold every table's indices in one array")
+        cap = sp.nnz_total if sp.include_last else sum(int(i.numel()) for i in sp.indices)
+        self._ensure_stage(max(int(cap), 1), sp.idx_bytes)
+        arr, st = self._host_desc(sp)
+        _lib.check(self.lib.dlrm_b200_host_stage_in(arr, len(self.host), C.byref(st), self.D, sp.batch, sp.idx_bytes,
+                                                    int(sp.include_last), _stream()), "host_stage_in")
+        self.n_launch += 2      # counter memset + kernel
+        self._staged, self._staged_by_link = sp, by_link
+
+    def _stage_out(self, write: bool):
+        """After the update: staged rows back to their host rows; forward only: release the slots."""
+        if self._staged is None:
+            return
+        arr, st = self._host_desc(self._staged)
+        self._staged = None
+        fn = self.lib.dlrm_b200_host_write_back if write else self.lib.dlrm_b200_host_release
+        _lib.check(fn(arr, len(self.host), C.byref(st), self.D, _stream()), "host_write_back")
+        self.n_launch += 1
+
+    def _abandon_staging(self):
+        """A step raised between stage-in and write-back: return the staged rows so that no slot stays claimed."""
+        if self.host and self._staged is not None:
+            with contextlib.suppress(Exception):
+                self._stage_out(True)
+
     def table(self, k: int) -> torch.Tensor:
-        """[rows_k, D] view of table k (strided when the accumulator is interleaved; fp16 with emb_dtype="fp16")."""
-        return self.tables[int(self.row_base[k]):int(self.row_base[k + 1]), :self.D]
+        """[rows_k, D] view of table k (strided when the accumulator is interleaved; fp16 with emb_dtype="fp16").
+        A host table's view is a CPU tensor of pinned memory, returned after the engine's work has completed."""
+        if self.is_host[k]:
+            self._host_sync()
+            return self._rows_of(self.tables_h, k)[:, :self.D]
+        return self._rows_of(self.tables, k)[:, :self.D]
+
+    def _rows_of(self, arena: torch.Tensor, k: int) -> torch.Tensor:
+        """Rows of table k in `arena` (a device arena or its host twin; the table decides which)."""
+        return arena[self._abase[k]:self._abase[k] + self.ln_emb[k]]
+
+    def momentum_of(self, k: int) -> Optional[torch.Tensor]:
+        """[rows_k] row-wise Adagrad accumulators of table k (a CPU view for a host table), or None."""
+        if self.is_host[k]:
+            self._host_sync()
+            m = (self.tables_h.view(torch.float32)[:, self._meta_col] if self.interleave else self._momentum_sep_h)
+        else:
+            m = self.momentum
+        return None if m is None else self._rows_of(m, k)
 
     @property
     def _meta_col(self) -> int:
@@ -399,24 +571,32 @@ class Engine:
     def ensure_optimizer_state(self, optimizer: str):
         if optimizer == "rwsadagrad":
             if not self.interleave and self._momentum_sep is None:
-                self._momentum_sep = torch.zeros(self.total_rows, dtype=torch.float32, device=self.device)
+                self._momentum_sep = torch.zeros(self.dev_rows, dtype=torch.float32, device=self.device)
+                if self.host:
+                    self._momentum_sep_h = self._pinned_zeros((self.host_rows,))
         if optimizer == "adagrad" and self.acc_ew is None:
             # One fp32 accumulator per table element (4 D bytes per row), in its own arena: the optimizer is created
             # after the tables are laid out (dlrm_s_pytorch.py builds DLRM_Net first), and moving the tables into an
             # interleaved [w | s] layout then would move every emb_l[k].weight.
-            self.acc_ew = torch.zeros((self.total_rows, self.D), dtype=torch.float32, device=self.device)
+            self.acc_ew = torch.zeros((self.dev_rows, self.D), dtype=torch.float32, device=self.device)
+            if self.host:
+                self.acc_ew_h = self._pinned_zeros((self.host_rows, self.D))
         if optimizer in _LR_DECAY and self.dense_state is None:
             self.dense_state = torch.zeros_like(self.dense)
 
     def accumulator_ew(self, k: int) -> torch.Tensor:
         """[rows_k, D] element-wise Adagrad accumulators of table k (after ensure_optimizer_state("adagrad"))."""
-        return self.acc_ew[int(self.row_base[k]):int(self.row_base[k + 1])]
+        if self.is_host[k]:
+            self._host_sync()
+            return self._rows_of(self.acc_ew_h, k)
+        return self._rows_of(self.acc_ew, k)
 
     def _point_at_acc_ew(self, desc, ks):
-        """Element-wise Adagrad: the descriptors of tables ks take the [rows, D] accumulator rows as `momentum`."""
+        """Element-wise Adagrad: the descriptors of tables ks take the [rows, D] accumulator rows as `momentum`
+        (a host table's: its staged rows)."""
         base = self.acc_ew.data_ptr()
         for n, k in enumerate(ks):
-            desc[n].momentum = base + int(self.row_base[k]) * self.D * 4
+            desc[n].momentum = self.stage_acc.data_ptr() if self.is_host[k] else base + self._abase[k] * self.D * 4
             desc[n].mom_stride = self.D
 
     # ------------------------------------------------------------------ parameters
@@ -428,6 +608,8 @@ class Engine:
         self._pack_dirty = True
         """params = dict(emb=[W_k], bot=[(W,b)...], top=[(W,b)...], v_W_l=None|[...]) of numpy /
         torch arrays (the layout of the oracle and of the reference's state_dict)."""
+        if self.host and params.get("v_W_l") is not None:
+            raise ValueError("host tables do not support weighted pooling: row_weights is indexed by the table row")
         with torch.no_grad():
             for k, Wk in enumerate(params["emb"]):     # fp16 tables: round to nearest
                 self.table(k).copy_(torch.as_tensor(Wk, dtype=torch.float32))
@@ -454,7 +636,15 @@ class Engine:
                 a = float(np.sqrt(1.0 / int(self.shards[k]["rows"])))      # the bound of the WHOLE table (:280-284)
                 tk = self.table(k)
                 for r0 in range(0, tk.shape[0], 1 << 24):                    # chunks: any temporary stays < 9 GB
-                    if self.f16:
+                    if self.is_host[k]:
+                        # the draw of a device engine: the same chunk of full rows (same sizes and row stride) on the
+                        # device, its other words kept, then copied back out whole
+                        hrows = self._rows_of(self.tables_h, k)[r0:r0 + (1 << 24)]
+                        tmp = hrows.to(self.device)
+                        tmp[:, :self.D].uniform_(-a, a, generator=g)
+                        hrows.copy_(tmp)
+                        del tmp
+                    elif self.f16:
                         # the fp32 draw of an fp32 engine, rounded to nearest.  The draw goes into a view with the
                         # fp32 engine's sizes AND row stride: torch's generator maps values to elements through the
                         # iteration space of its output (split into 32-bit-indexable pieces by the byte span), so
@@ -479,7 +669,7 @@ class Engine:
         for n, k in enumerate(ks):
             d = arr[n]
             sh = self.shards[k]
-            d.weight = self.tables.data_ptr() + int(self.row_base[k]) * self.ldw * self.esize
+            d.weight = self.tables.data_ptr() + self._abase[k] * self.ldw * self.esize
             d.ld = self.ldw
             d.weight_dtype = DTYPE_F16 if self.f16 else DTYPE_F32
             d.indices = sp.indices[k].data_ptr() if sp.indices[k].numel() else 0
@@ -489,6 +679,9 @@ class Engine:
             d.nnz = sp.indices[k].numel()
             d.rows = int(sh["rows"])
             d.row_lo, d.row_n = int(sh["row_lo"]), int(sh["row_n"])
+            if self.is_host[k]:      # the staged rows, read through the slot of every position
+                d.weight, d.indices = self.stage_w.data_ptr(), self._slot_ptr(sp, k)
+                d.rows, d.row_lo, d.row_n = self.stage_cap, 0, self.stage_cap
             if route is not None:
                 d.out_off, d.out_stride = int(route[k][0]), int(route[k][1])
         return arr
@@ -503,7 +696,9 @@ class Engine:
             d.row_lo, d.row_n = int(sh["row_lo"]), int(sh["row_n"])
             if dy_off is not None:
                 d.use_dy_off, d.dy_off = 1, int(dy_off[k])
-            d.weight = self.tables.data_ptr() + int(self.row_base[k]) * self.ldw * self.esize
+            d.weight = self.tables.data_ptr() + self._abase[k] * self.ldw * self.esize
+            if self.is_host[k]:
+                d.weight, d.row_lo, d.row_n = self.stage_w.data_ptr(), 0, self.stage_cap
             d.ld = self.ldw
             if self.f16:
                 d.weight_dtype = DTYPE_F16
@@ -512,21 +707,27 @@ class Engine:
                 d.momentum = d.weight + self.D * self.esize
                 d.mom_stride = self.ldw * self.esize // 4
             else:
-                d.momentum = (self._momentum_sep.data_ptr() + int(self.row_base[k]) * 4
+                d.momentum = (self._momentum_sep.data_ptr() + self._abase[k] * 4
                               if self._momentum_sep is not None else None)
+                if self.is_host[k]:
+                    d.momentum = self.stage_mom.data_ptr() if self._momentum_sep is not None else None
                 d.mom_stride = 1
             # tiny tables are neither linked nor list-updated (head NULL): emb_small_update handles them
             if self.is_small(k):
                 d.head = None
             elif self.interleave:
                 d.head, d.head_stride = d.weight + self.D * self.esize + 4, self.ldw * self.esize // 4
+            elif self.is_host[k]:
+                d.head, d.head_stride = self.stage_head.data_ptr(), 1
             else:
-                d.head, d.head_stride = self._head_sep.data_ptr() + int(self.row_base[k]) * 4, 1
+                d.head, d.head_stride = self._head_sep.data_ptr() + self._abase[k] * 4, 1
             d.mark = self.mark.data_ptr() if self.mark is not None else None
             d.indices = sp.indices[k].data_ptr() if sp.indices[k].numel() else 0
             d.offsets = sp.offsets[k].data_ptr()
             d.nnz = sp.indices[k].numel()
             d.rows = int(sh["rows"])
+            if self.is_host[k]:
+                d.indices, d.rows = self._slot_ptr(sp, k), self.stage_cap
             d.pair_base = 0 if sp.include_last else base
             base += sp.indices[k].numel()
         total = sp.nnz_total if sp.include_last else base
@@ -549,6 +750,10 @@ class Engine:
         if link:
             total = sp.nnz_total if sp.include_last else sum(int(i.numel()) for i in sp.indices)
             self._ensure_link(total)
+        # host tables: stage the rows first (unless emb_link already staged this batch for its update)
+        stage = bool(self.host) and not (self._staged is sp and self._staged_by_link)
+        if stage:
+            self._stage_in(sp)
         routed = out is None
         route = self.route_out if routed else [(k * stride_table, stride_sample) for k in range(self.T)]
         whole = [k for k in range(self.T) if int(self.shards[k]["nparts"]) == 1]
@@ -587,6 +792,8 @@ class Engine:
             self._filtered = use_filter
             if use_filter:
                 self.emb_classify(sp)
+        elif stage:
+            self._stage_out(False)      # forward only: nothing will update the staged rows
 
     def mlp_forward(self, which: str, x: torch.Tensor, ldx: int, B: int, outs: List[torch.Tensor],
                     lds: List[int], upto: Optional[int] = None):
@@ -681,6 +888,9 @@ class Engine:
             self._alloc_activations(B)
         if train and self.T:
             self._ensure_link(sp.nnz_total if sp.include_last else sum(int(i.numel()) for i in sp.indices))
+        if self.host:
+            self._ensure_stage(max(int(sp.nnz_total if sp.include_last else sum(int(i.numel()) for i in sp.indices)),
+                                   1), sp.idx_bytes)
         if self.has_head:
             nt = len(self.ln_top) - 1
             need = int(self.lib.dlrm_b200_head_scratch_bytes(B, self.ln_top[nt - 1]))
@@ -705,6 +915,8 @@ class Engine:
         issued on a side stream, concurrently with the forward pass."""
         total = sp.nnz_total if sp.include_last else sum(int(i.numel()) for i in sp.indices)
         self._ensure_link(total)
+        if self.host and self._staged is not sp:
+            self._stage_in(sp, by_link=True)
         for c0 in range(0, self.T, _lib.MAX_TABLES):
             ks = list(range(c0, min(self.T, c0 + _lib.MAX_TABLES)))
             desc, _ = self._bwd_desc_chunk(sp, ks)
@@ -734,6 +946,8 @@ class Engine:
         base = None if peer is not None else (self.dT.data_ptr() if routed else dY.data_ptr())
         big = [k for k in range(self.T) if not self.is_small(k)]
         small = [k for k in range(self.T) if self.is_small(k)]
+        if self.host and self._staged is not sp:
+            raise RuntimeError("host tables: emb_update needs this batch staged by forward(link=True) or emb_link()")
         # The tiny-table kernels (few, long-running CTAs) go FIRST, on their own stream: they take their SM slots and the
         # grid-stride list-path update fills the rest of the machine beside them (different tables, no ordering needed).
         side = bool(small) and bool(big) and os.environ.get("DLRM_SMALL_SIDE", "1") != "0"
@@ -771,6 +985,8 @@ class Engine:
                                                              int(sp.include_last), self.link.data_ptr(), base, ss, 0,
                                                              _OPT[optimizer], lr, eps, dd, _stream()), "emb_bwd_update")
             self.n_launch += 1
+        if self.host:
+            self._stage_out(True)       # same stream as the update: the rows go home before anything reads them
         if side:
             self._join(self.s_small)
 
@@ -945,15 +1161,19 @@ class Engine:
         reading the tables from another stream."""
         self.ensure_optimizer_state(optimizer)
         self._join_update = bool(join_update) or not self.tc
-        self.forward(X, sp, link=not link_done, skip_head=True)
-        self.opt_step += 1
-        clr = lr / (1.0 + (self.opt_step - 1.0) * lr_decay) if optimizer in _LR_DECAY else lr
-        if self.tc:
-            self.backward(X, sp, target, update=(optimizer, clr))
-        else:
-            self.backward(X, sp, target)
-            if self.T:
-                self.emb_update(sp, optimizer=optimizer, lr=clr)
+        try:
+            self.forward(X, sp, link=not link_done, skip_head=True)
+            self.opt_step += 1
+            clr = lr / (1.0 + (self.opt_step - 1.0) * lr_decay) if optimizer in _LR_DECAY else lr
+            if self.tc:
+                self.backward(X, sp, target, update=(optimizer, clr))
+            else:
+                self.backward(X, sp, target)
+                if self.T:
+                    self.emb_update(sp, optimizer=optimizer, lr=clr)
+        except BaseException:
+            self._abandon_staging()
+            raise
         self.dense_apply(optimizer, clr)
         return self.loss_buf
 
@@ -980,12 +1200,16 @@ class Engine:
         """optimizer.step() on the gradients the last backward() left in the engine's buffers: embedding rows
         (through the sharded exchange when there is one), then the dense parameters."""
         if self.T or self.update_fn is not None:
-            if not linked and self.T:
-                self.emb_link(sp)
-            if self.update_fn is not None:
-                self.update_fn(sp, optimizer, clr)
-            else:
-                self.emb_update(sp, optimizer=optimizer, lr=clr, eps=eps)
+            try:
+                if not linked and self.T:
+                    self.emb_link(sp)
+                if self.update_fn is not None:
+                    self.update_fn(sp, optimizer, clr)
+                else:
+                    self.emb_update(sp, optimizer=optimizer, lr=clr, eps=eps)
+            except BaseException:
+                self._abandon_staging()
+                raise
         self.dense_apply(optimizer, clr, eps)
 
     # ================================================================== wgmma path
@@ -1316,6 +1540,15 @@ class Engine:
         if update is not None and has_emb and getattr(self, "_join_update", True):
             self._join(self.s_emb)
             self._mark("join_update")
+
+
+def _unpin(lib, tensors):
+    """Unregister the pinned host arenas of a collected engine (after its last staging copy)."""
+    with contextlib.suppress(Exception):
+        torch.cuda.synchronize()
+    for t in tensors:
+        with contextlib.suppress(Exception):
+            lib.dlrm_b200_host_unregister(t.data_ptr())
 
 
 def _refuse_graphed_f16(eng: "Engine"):

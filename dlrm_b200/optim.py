@@ -78,7 +78,7 @@ class _Fused(torch.optim.Optimizer):
             if eng.table(k).data_ptr() == p.data_ptr():
                 if self._name == "adagrad":
                     return "sum", eng.accumulator_ew(k)
-                return "momentum", eng.momentum[int(eng.row_base[k]):int(eng.row_base[k + 1])]
+                return "momentum", eng.momentum_of(k)
         raise RuntimeError("parameter is not backed by the engine's memory")
 
     def state_dict(self):

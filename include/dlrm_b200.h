@@ -513,6 +513,64 @@ int dlrm_b200_ingest_records(const void* x_int, int x_int_dtype, const void* x_c
                              int32_t* ring_cat, int32_t* ring_y, int64_t capacity, int64_t dst, uint64_t* bad,
                              void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Host tables (csrc/host_tables.cu): fp32 tables whose rows live in pinned, mapped host memory.  The rows a batch
+ * touches are staged into an HBM arena before the gather and written back after the update, so the gather and
+ * update entry points above run unchanged on the staging arena (rows = capacity) with `slot_idx` as their indices.
+ *   stage_in   : for every occurrence p (global position: pos_base + local position; a packed batch's offsets are
+ *                already global, pos_base 0) of a host table, over the positions the gather reads
+ *                ([offsets[0], end of the last bag)): an index outside [0, rows) sets the device error word and
+ *                writes slot -1 (the gather then reports and skips it as well); otherwise the first occurrence of
+ *                its row claims map[row] (0 -> p + 1), becomes the row's slot p, and copies the row (ld floats,
+ *                the word head_col written as zero), its separate accumulator and its element-wise Adagrad row
+ *                into slot p of the staging arrays.  slot_idx[p] = the slot, in the batch's index dtype.  The
+ *                counter is reset by a memset on `stream` first; it ends as the number of distinct rows, and
+ *                list[0 .. count) holds their slots.
+ *   write_back : every listed slot back to its host row (head_col written as zero), and map[row] = 0.
+ *   release    : map[row] = 0 for every listed slot only (a forward without an update).
+ * The map of a table is int32 [rows], all zero between steps; untouched host rows are never read or written.
+ * Host pointers must be device-accessible at the same address (unified addressing; dlrm_b200_host_register).
+ * The tables of one call share the row layout: ld floats per row (dim when 0), separate accumulators either for
+ * every table and the staging or for none, and the same for element-wise accumulators ([rows][dim]).
+ * ------------------------------------------------------------------------------------------ */
+typedef struct {
+  float* weight;        /* [host] rows [rows][ld] */
+  float* momentum;      /* [host] separate row-wise accumulators [rows], or NULL */
+  float* acc_ew;        /* [host] element-wise Adagrad accumulators [rows][dim], or NULL */
+  const void* indices;  /* as in dlrm_emb_fwd_table_t */
+  const void* offsets;
+  int64_t nnz;
+  int64_t rows;
+  int64_t pos_base;     /* first global position of this table (reference format: pair_base) */
+  int32_t* map;         /* [rows] device, zero between steps */
+} dlrm_host_table_t;
+
+typedef struct {
+  float* weight;        /* [capacity][ld] */
+  float* momentum;      /* [capacity] or NULL */
+  int32_t* head;        /* [capacity] separate list heads, set to zero for every staged slot, or NULL */
+  float* acc_ew;        /* [capacity][dim] or NULL */
+  void* slot_idx;       /* [capacity] slot of every position, the batch's index dtype */
+  int32_t* list;        /* [capacity] staged slots */
+  int64_t* key;         /* [capacity] row * 64 + table of a staged slot */
+  int32_t* count;       /* one int32: staged rows */
+  int64_t capacity;     /* positions (and slots); every global position must be below it */
+  int64_t ld;           /* floats per row; 0 = dim */
+  int64_t head_col;     /* word of the row holding the list head (interleaved rows), or -1 */
+} dlrm_host_stage_t;
+
+int dlrm_b200_host_stage_in(const dlrm_host_table_t* tables /*[host]*/, int num_tables,
+                            const dlrm_host_stage_t* stage /*[host]*/, int dim, int64_t batch, int idx_bytes,
+                            int include_last, void* stream);
+int dlrm_b200_host_write_back(const dlrm_host_table_t* tables /*[host]*/, int num_tables,
+                              const dlrm_host_stage_t* stage /*[host]*/, int dim, void* stream);
+int dlrm_b200_host_release(const dlrm_host_table_t* tables /*[host]*/, int num_tables,
+                           const dlrm_host_stage_t* stage /*[host]*/, int dim, void* stream);
+/* Page-lock [ptr, ptr + bytes) of ordinary host memory as mapped memory (cudaHostRegister) and check that the
+ * device address equals ptr; error (and nothing stays registered) otherwise.  Synchronous. */
+int dlrm_b200_host_register(void* ptr, int64_t bytes);
+int dlrm_b200_host_unregister(void* ptr);
+
 #ifdef __cplusplus
 }
 #endif
