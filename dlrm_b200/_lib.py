@@ -52,7 +52,11 @@ class HostTable(C.Structure):
 class HostStage(C.Structure):
     _fields_ = [("weight", C.c_void_p), ("momentum", C.c_void_p), ("head", C.c_void_p), ("acc_ew", C.c_void_p),
                 ("slot_idx", C.c_void_p), ("list", C.c_void_p), ("key", C.c_void_p), ("count", C.c_void_p),
-                ("capacity", C.c_int64), ("ld", C.c_int64), ("head_col", C.c_int64)]
+                ("capacity", C.c_int64), ("ld", C.c_int64), ("head_col", C.c_int64),
+                # row cache (all zero: none)
+                ("cache_rows", C.c_int64), ("cache_tag", C.c_void_p), ("cache_used", C.c_void_p), ("step", C.c_void_p),
+                ("set_head", C.c_void_p), ("set_next", C.c_void_p), ("sets", C.c_void_p), ("num_sets", C.c_void_p),
+                ("stats", C.c_void_p), ("forward_only", C.c_int64)]
 
 
 class GemmTcDesc(C.Structure):
@@ -96,7 +100,7 @@ SYMBOLS = [
     "dlrm_b200_block_copy", "dlrm_b200_gen_multihot", "dlrm_b200_set_tunable", "dlrm_b200_emb_bag_fwd_remote", "dlrm_b200_split_bf16", "dlrm_b200_dense_update_pack",
     "dlrm_b200_decode_records", "dlrm_b200_gather_records", "dlrm_b200_ingest_records",
     "dlrm_b200_host_stage_in", "dlrm_b200_host_write_back", "dlrm_b200_host_release", "dlrm_b200_host_register",
-    "dlrm_b200_host_unregister",
+    "dlrm_b200_host_unregister", "dlrm_b200_host_cache_flush",
 ]
 
 
@@ -159,6 +163,7 @@ def _declare(lib):
     lib.dlrm_b200_host_stage_in.argtypes = [C.POINTER(HostTable), i32, C.POINTER(HostStage), i32, i64, i32, i32, vp]
     lib.dlrm_b200_host_write_back.argtypes = [C.POINTER(HostTable), i32, C.POINTER(HostStage), i32, vp]
     lib.dlrm_b200_host_release.argtypes = [C.POINTER(HostTable), i32, C.POINTER(HostStage), i32, vp]
+    lib.dlrm_b200_host_cache_flush.argtypes = [C.POINTER(HostTable), i32, C.POINTER(HostStage), i32, vp]
     lib.dlrm_b200_host_register.argtypes = [vp, i64]
     lib.dlrm_b200_host_unregister.argtypes = [vp]
     for name in SYMBOLS:

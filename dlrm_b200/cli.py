@@ -102,6 +102,9 @@ def build_parser():
     # dlrm_b200 addition: tables kept in pinned host memory, their touched rows staged through HBM every step
     # ("" none, "auto": the largest tables until the rest fits in device memory, or dash-separated table ids)
     p.add_argument("--emb-host-tables", type=str, default="")
+    # dlrm_b200 addition: rows of the host tables kept in HBM between steps ("" none, "auto": the device memory left
+    # free beyond the reserve of --emb-host-tables=auto, or a row count)
+    p.add_argument("--emb-host-cache", type=str, default="")
     return p
 
 
@@ -406,6 +409,20 @@ def run(argv=None):
                          % (tiny[0], int(ln_emb[tiny[0]])))
         if host_tables == "auto" and args.optimizer == "adagrad":
             host_tables = _auto_adagrad(ln_emb, m_spa, device)
+    host_cache = None
+    if args.emb_host_cache:
+        from . import host_tables as ht
+
+        if not host_tables:
+            sys.exit("ERROR: --emb-host-cache needs --emb-host-tables (the cache holds rows of host tables)")
+        try:
+            host_cache = ht.parse_cache(args.emb_host_cache)
+            if host_cache != "auto":
+                lookups = args.num_indices_per_lookup if args.data_generation == "random" else 1
+                ht.check_cache_size(host_cache, max(args.mini_batch_size, args.test_mini_batch_size)
+                                    * ln_emb.size * lookups)
+        except ValueError as e:
+            sys.exit("ERROR: " + str(e))
     dlrm = DLRM_Net(m_spa, ln_emb, ln_bot, ln_top, arch_interaction_op=args.arch_interaction_op,
                     arch_interaction_itself=args.arch_interaction_itself, sigmoid_bot=-1,
                     sigmoid_top=ln_top.size - 2, sync_dense_params=args.sync_dense_params,
@@ -413,7 +430,7 @@ def run(argv=None):
                     loss_function=args.loss_function, device=device, gemm=args.gemm,
                     max_batch=args.mini_batch_size, loss_weights=loss_ws,
                     emb_dtype=torch.float16 if args.emb_dtype == "fp16" else torch.float32,
-                    emb_host_tables=host_tables or None)
+                    emb_host_tables=host_tables or None, emb_host_cache=host_cache or None)
     optimizer = lr_scheduler = None
     if not args.inference_only:
         opts = {"sgd": fused.SGD, "rwsadagrad": fused.RWSAdagrad, "adagrad": fused.Adagrad}   # :1342-1346

@@ -22,7 +22,11 @@ then holds fp16 tables; an fp32 checkpoint loads with round-to-nearest, an fp16 
 `emb_host_tables="auto" | [k, ...]` keeps those tables in pinned host memory (dlrm_b200/host_tables.py): their
 `emb_l[k].weight` are CPU tensors, so `state_dict()` / `load_state_dict()` and checkpoints are unchanged, and every step
 stages the rows the batch touches through HBM.  "auto" moves the largest tables until the rest fits in free device
-memory.  QR / mixed-dimension embeddings, quantised embeddings and `parallel_forward` are outside the path
+memory.  `emb_host_cache=N | "auto"` also keeps up to N of their rows in HBM between steps (a 32-way set-associative
+cache, least recently used way replaced; "auto": the device memory free at the first batch beyond `host_reserve`).
+A cached row's host copy is then stale: `emb_l[k].weight` of a host table shows the current rows only after
+`state_dict()`, `load_state_dict()`, `engine.table(k)` or the optimizer's `state_dict()`, which write the cache back
+(and empty it).  A training loop that calls none of them never writes it back.  QR / mixed-dimension embeddings, quantised embeddings and `parallel_forward` are outside the path
 (SURVEY §2) and exit with an error when requested.
 """
 from __future__ import annotations
@@ -122,7 +126,7 @@ class DLRM_Net(nn.Module):
                  loss_threshold=0.0, ndevices=-1, qr_flag=False, qr_operation="mult", qr_collisions=0,
                  qr_threshold=200, md_flag=False, md_threshold=200, weighted_pooling=None,
                  loss_function="bce", *, device=None, gemm="tc", max_batch=2048, loss_weights=None,
-                 emb_dtype=torch.float32, round_seed=0, emb_host_tables=None):
+                 emb_dtype=torch.float32, round_seed=0, emb_host_tables=None, emb_host_cache=None):
         super().__init__()
         self._engine: Optional[Engine] = None
         self._fused_opt = None
@@ -192,6 +196,8 @@ class DLRM_Net(nn.Module):
                     sys.exit("ERROR: " + str(e))
             else:
                 host = sorted(set(int(k) for k in emb_host_tables))
+        if emb_host_cache and not host:
+            sys.exit("ERROR: a host row cache (emb_host_cache) needs host embedding tables (emb_host_tables)")
 
         if tdist.is_available() and tdist.is_initialized() and tdist.get_world_size() > 1:
             # one process per GPU (the reference: ext_dist.my_size > 1, dlrm_s_pytorch.py:352-365): tables are
@@ -216,7 +222,9 @@ class DLRM_Net(nn.Module):
                                   sigmoid_bot=sigmoid_bot, sigmoid_top=sigmoid_top, loss=loss_function,
                                   loss_threshold=loss_threshold, loss_ws=loss_ws, device=device,
                                   max_batch=max_batch, gemm=gemm, emb_dtype=emb_dtype, round_seed=round_seed,
-                                  interleave_momentum=None if emb_dtype == "fp16" else False, host_tables=host)
+                                  interleave_momentum=None if emb_dtype == "fp16" else False, host_tables=host,
+                                  host_cache_rows=emb_host_cache or 0,
+                                  host_cache_reserve=self.host_reserve(m_spa, ln_emb))
         self._m_spa, self._ln_emb = int(m_spa), ln_emb
         # same construction (and numpy RNG consumption) order as the reference: tables, bottom, top
         if ndevices <= 1:

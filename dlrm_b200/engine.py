@@ -28,6 +28,7 @@ from __future__ import annotations
 import contextlib
 import ctypes as C
 import os
+import warnings
 from dataclasses import dataclass
 from typing import List, Optional, Sequence
 
@@ -100,7 +101,8 @@ class Engine:
                  loss: str = "bce", loss_threshold: float = 0.0, loss_ws=None, device="cuda:0",
                  max_batch: int = 2048, gemm: str = "simt", n_features: Optional[int] = None,
                  interleave_momentum: Optional[bool] = None, shards=None, split_slots=None, small_rows_max: int = 256,
-                 emb_dtype: str = "fp32", round_seed: int = 0, host_tables: Sequence[int] = ()):
+                 emb_dtype: str = "fp32", round_seed: int = 0, host_tables: Sequence[int] = (),
+                 host_cache_rows=0, host_cache_reserve: int = 1 << 31):
         if not torch.cuda.is_available():
             raise RuntimeError("dlrm_b200.Engine needs a CUDA device (H100, sm_90a); there is no CPU path")
         self.device = torch.device(device)
@@ -182,6 +184,7 @@ class Engine:
         self.host = sorted(set(int(k) for k in host_tables))
         self.is_host = [k in self.host for k in range(self.T)]
         self._check_host_tables(interleave_momentum)
+        self._check_host_cache(host_cache_rows, host_cache_reserve)
         self._abase, nb = [], [0, 0]
         for k, n in enumerate(self.ln_emb):
             self._abase.append(nb[self.is_host[k]])
@@ -408,6 +411,24 @@ class Engine:
                              "two-pass update, which indexes the whole table on the device"
                              % (tiny[0], self.ln_emb[tiny[0]], self.small_rows_max))
 
+    def _check_host_cache(self, rows, reserve):
+        """Row cache of the host tables (host_cache_rows: 0 = none, "auto", or a row count rounded up to 32)."""
+        from .host_tables import MAP_LIMIT
+
+        self.cache_rows = 0
+        self._cache_auto = rows == "auto"
+        self._cache_reserve = int(reserve)
+        if not self._cache_auto:
+            rows = int(rows)
+            if rows < 0:
+                raise ValueError("host_cache_rows=%d: expected 0 (no cache), a row count or \"auto\"" % rows)
+            self.cache_rows = (rows + 31) // 32 * 32
+        if (self._cache_auto or self.cache_rows) and not self.host:
+            raise ValueError("host_cache_rows: a host row cache needs host tables (host_tables=[...])")
+        if self.cache_rows + 1 > MAP_LIMIT:
+            raise ValueError("host_cache_rows=%d: cache rows + staging positions must fit the int32 slot map (<= %d)"
+                             % (self.cache_rows, MAP_LIMIT))
+
     def _pinned_zeros(self, shape) -> torch.Tensor:
         """Zeros in page-locked host memory mapped at the same device address (cudaHostRegister on a plain CPU tensor:
         torch's pinned allocator would round every block up to a power of two)."""
@@ -425,7 +446,12 @@ class Engine:
         self.tables_h = self._momentum_sep_h = self.acc_ew_h = None
         self._staged = None             # SparseInput whose host-table rows are in the staging arena
         self._staged_by_link = False
+        self._staged_train = False
         self.stage_cap = 0
+        self._arena_rows = 0            # cache rows + staging positions of the device arena
+        self._cache_ready = False
+        self._cache_dirty = False       # a training step may have left rows in the cache since the last flush
+        self.cache_flushes = 0
         if not self.host:
             return
         import weakref
@@ -442,24 +468,93 @@ class Engine:
         weakref.finalize(self, _unpin, self.lib, self._pinned)
 
     def _host_sync(self):
-        """Host reads and writes of host rows wait for every staging copy the engine has enqueued."""
+        """Host reads and writes of host rows wait for every staging copy the engine has enqueued.  With a row cache,
+        every resident row is written back and the cache emptied first: the caller sees current rows, and whatever it
+        writes through its view is what the next step stages.  The flush waits for every stream first (an insert may
+        still run on the update's stream), and runs only if a training step ran since the last one."""
         torch.cuda.synchronize(self.device)
+        if self._cache_dirty:
+            self._flush_cache()
+            torch.cuda.synchronize(self.device)
+
+    def _flush_cache(self):
+        """Every resident row back to host memory and the cache emptied (current stream; the caller has ordered it
+        after the last insert)."""
+        arr, st = self._host_desc(None)
+        _lib.check(self.lib.dlrm_b200_host_cache_flush(arr, len(self.host), C.byref(st), self.D, _stream()),
+                   "host_cache_flush")
+        self.n_launch += 1
+        self.cache_flushes += 1
+        self._cache_dirty = False
+
+    def _cache_row_bytes(self) -> int:
+        """Device bytes of one cache row: its arena row and words, tag (8), last use (4), set lists (< 1)."""
+        return (4 * self.ldw + (0 if self.interleave else 4) + (4 if self._momentum_sep_h is not None else 0)
+                + (4 * self.D if self.acc_ew_h is not None else 0) + 13)
+
+    def _init_cache(self, cap: int):
+        """Size ("auto": from the free device memory when the first batch is staged, beside a staging arena of `cap`
+        positions) and allocate the cache's metadata, once, before the first arena is laid out."""
+        from .host_tables import auto_cache_rows
+
+        dev = self.device
+        if self._cache_auto:
+            free, _ = torch.cuda.mem_get_info(dev)
+            row = self._cache_row_bytes()
+            stage = cap * (row - 13 + 4 + 8 + 8)        # arena rows, list, key, slot indices
+            self.cache_rows = auto_cache_rows(free - stage, self._cache_reserve, row, self.host_rows)
+            self._cache_auto = False
+        N = self.cache_rows
+        if N:
+            self.cache_tag = torch.full((N,), -1, dtype=torch.int64, device=dev)
+            self.cache_used = torch.zeros(N, dtype=torch.int32, device=dev)
+            self.cache_step = torch.zeros(1, dtype=torch.int32, device=dev)
+            self.cache_set_head = torch.zeros(N // 32, dtype=torch.int32, device=dev)
+            self.cache_sets = torch.zeros(N // 32, dtype=torch.int32, device=dev)
+            self.cache_nsets = torch.zeros(1, dtype=torch.int32, device=dev)
+            self.cache_stats = torch.zeros(4, dtype=torch.int64, device=dev)
+            self._cache_ready = True
 
     def _ensure_stage(self, cap: int, idx_bytes: int):
-        """Staging arena for `cap` positions (one slot per position of the batch)."""
+        """Device arena for the cache rows and `cap` staging positions (one slot per position of the batch).  When
+        the staging grows, the cache is written back and emptied and the old arena released before the new one is
+        allocated: there is never a second copy of the cache rows, so an "auto" cache sized at the first batch
+        still fits when a later batch needs more staging."""
+        from .host_tables import MAP_LIMIT
+
         dev = self.device
+        if not self._cache_ready and (self._cache_auto or self.cache_rows):
+            self._init_cache(cap)
+        N = self.cache_rows
         if cap > self.stage_cap:
+            if N + cap > MAP_LIMIT:
+                raise ValueError("host tables: %d cache rows + %d staging positions do not fit the int32 slot map "
+                                 "(<= %d)" % (N, cap, MAP_LIMIT))
+            if N and self.stage_cap:
+                if self._staged is not None:
+                    self._stage_out(True)
+                torch.cuda.synchronize(self.device)       # inserts on the update's stream have finished
+                if self._cache_dirty:
+                    self._flush_cache()
+                self.stage_w = self.stage_head = self.stage_mom = self.stage_acc = None
+            if N and cap > 256 * (N // 32):
+                warnings.warn("host cache of %d rows: %d sets for up to %d misses per step; one warp walks each "
+                              "set's misses, so a step can be slower than without the cache (use at least %d rows)"
+                              % (N, N // 32, cap, (cap + 255) // 256 * 32), stacklevel=3)
             self.stage_cap = cap
-            self.stage_w = torch.zeros((cap, self.ldw), dtype=torch.float32, device=dev)
-            self.stage_head = None if self.interleave else torch.zeros(cap, dtype=torch.int32, device=dev)
+            self._arena_rows = N + cap
+            self.stage_w = torch.zeros((N + cap, self.ldw), dtype=torch.float32, device=dev)
+            self.stage_head = None if self.interleave else torch.zeros(N + cap, dtype=torch.int32, device=dev)
             self.stage_list = torch.zeros(cap, dtype=torch.int32, device=dev)
             self.stage_key = torch.zeros(cap, dtype=torch.int64, device=dev)
             self.stage_mom = self.stage_acc = None
             self._slot_idx = {}
+            if N:
+                self.cache_set_next = torch.zeros(cap, dtype=torch.int32, device=dev)
         if self._momentum_sep_h is not None and self.stage_mom is None:
-            self.stage_mom = torch.zeros(self.stage_cap, dtype=torch.float32, device=dev)
+            self.stage_mom = torch.zeros(self._arena_rows, dtype=torch.float32, device=dev)
         if self.acc_ew_h is not None and self.stage_acc is None:
-            self.stage_acc = torch.zeros((self.stage_cap, self.D), dtype=torch.float32, device=dev)
+            self.stage_acc = torch.zeros((self._arena_rows, self.D), dtype=torch.float32, device=dev)
         if idx_bytes not in self._slot_idx:
             dt = torch.int64 if idx_bytes == 8 else torch.int32
             self._slot_idx[idx_bytes] = torch.zeros(self.stage_cap, dtype=dt, device=dev)
@@ -472,7 +567,8 @@ class Engine:
     def _slot_ptr(self, sp: SparseInput, k: int) -> int:
         return self._slot_idx[sp.idx_bytes].data_ptr() + self._pos_base(sp, k) * sp.idx_bytes
 
-    def _host_desc(self, sp: SparseInput):
+    def _host_desc(self, sp: Optional[SparseInput], forward_only: bool = False):
+        """Descriptors of the host tables and the arena for batch `sp` (None: no batch, for the cache flush)."""
         arr = (_lib.HostTable * len(self.host))()
         for n, k in enumerate(self.host):
             d = arr[n]
@@ -483,6 +579,9 @@ class Engine:
                 d.acc_ew = self.acc_ew_h.data_ptr() + self._abase[k] * self.D * 4
             d.rows = self.ln_emb[k]
             d.map = self.slot_map.data_ptr() + self._map_base[k] * 4
+            if sp is None:
+                d.offsets = self.stage_count.data_ptr()        # never read
+                continue
             d.indices = sp.indices[k].data_ptr() if sp.indices[k].numel() else 0
             d.offsets = sp.offsets[k].data_ptr()
             d.nnz = sp.indices[k].numel()
@@ -494,12 +593,22 @@ class Engine:
         st.head = _ptr(self.stage_head)
         st.count, st.capacity, st.ld = self.stage_count.data_ptr(), self.stage_cap, self.ldw
         st.head_col = self._meta_col + 1 if self.interleave else -1
-        st.slot_idx = self._slot_idx[sp.idx_bytes].data_ptr()
+        st.slot_idx = next(iter(self._slot_idx.values())).data_ptr() if sp is None else \
+            self._slot_idx[sp.idx_bytes].data_ptr()
+        if self.cache_rows:
+            st.cache_rows, st.cache_tag, st.cache_used = self.cache_rows, self.cache_tag.data_ptr(), \
+                self.cache_used.data_ptr()
+            st.step, st.set_head, st.set_next = self.cache_step.data_ptr(), self.cache_set_head.data_ptr(), \
+                self.cache_set_next.data_ptr()
+            st.sets, st.num_sets, st.stats = self.cache_sets.data_ptr(), self.cache_nsets.data_ptr(), \
+                self.cache_stats.data_ptr()
+            st.forward_only = int(forward_only)
         return arr, st
 
-    def _stage_in(self, sp: SparseInput, by_link: bool = False):
+    def _stage_in(self, sp: SparseInput, by_link: bool = False, train: bool = True):
         """Stage the rows of this batch's host-table occurrences (current stream).  A staging left by a step that did
-        not finish is written back first (its rows are unchanged or updated; either way they go home)."""
+        not finish is written back first (its rows are unchanged or updated; either way they go home).  train=False:
+        a pass without an update, which leaves the row cache as it is."""
         if self.use_filter:
             raise ValueError("host tables do not support the duplicate filter (use_filter)")
         if self.row_weights is not None:
@@ -510,27 +619,52 @@ class Engine:
             raise ValueError("host tables: a packed batch must hold every table's indices in one array")
         cap = sp.nnz_total if sp.include_last else sum(int(i.numel()) for i in sp.indices)
         self._ensure_stage(max(int(cap), 1), sp.idx_bytes)
-        arr, st = self._host_desc(sp)
+        arr, st = self._host_desc(sp, forward_only=not train)
         _lib.check(self.lib.dlrm_b200_host_stage_in(arr, len(self.host), C.byref(st), self.D, sp.batch, sp.idx_bytes,
                                                     int(sp.include_last), _stream()), "host_stage_in")
-        self.n_launch += 2      # counter memset + kernel
-        self._staged, self._staged_by_link = sp, by_link
+        self.n_launch += 2      # counter memset (with a cache, a training pass: begin kernel) + kernel
+        if self.cache_rows and train:
+            self._cache_dirty = True
+        self._staged, self._staged_by_link, self._staged_train = sp, by_link, train
 
     def _stage_out(self, write: bool):
         """After the update: staged rows back to their host rows; forward only: release the slots."""
         if self._staged is None:
             return
-        arr, st = self._host_desc(self._staged)
+        if self.cache_rows and not self._staged_train:
+            write = False       # a pass without an update changed no row, and its misses are not cache candidates
+        arr, st = self._host_desc(self._staged, forward_only=not self._staged_train)
         self._staged = None
         fn = self.lib.dlrm_b200_host_write_back if write else self.lib.dlrm_b200_host_release
         _lib.check(fn(arr, len(self.host), C.byref(st), self.D, _stream()), "host_write_back")
-        self.n_launch += 1
+        self.n_launch += 2 if write and self.cache_rows else 1      # with a cache: insert kernel + write-back
 
     def _abandon_staging(self):
-        """A step raised between stage-in and write-back: return the staged rows so that no slot stays claimed."""
+        """A step raised between stage-in and write-back: return the staged rows so that no slot stays claimed.  With
+        a cache the misses are inserted as after an update (their rows are current either way), and the list heads of
+        the cache slots are cleared, since a link may have set them for an update that never ran."""
         if self.host and self._staged is not None:
             with contextlib.suppress(Exception):
                 self._stage_out(True)
+                if self.cache_rows:
+                    N = self.cache_rows
+                    if self.interleave:
+                        self.stage_w[:N, self._meta_col + 1].zero_()
+                    else:
+                        self.stage_head[:N].zero_()
+
+    def host_cache_stats(self) -> dict:
+        """Cumulative counters of the host row cache (synchronises): hits, inserts, evictions and staged (uncached)
+        rows, each per distinct row of a training step; plus the cache size, the training steps seen and the flushes
+        (a read of a host table's memory through table(k), momentum_of(k), accumulator_ew(k) or the module's
+        state_dict / load_state_dict writes the cache back when a training step ran since the last flush; so does a
+        growth of the staging arena).  All zero without a cache."""
+        out = dict(hits=0, inserts=0, evictions=0, staged=0, rows=self.cache_rows, steps=0,
+                   flushes=self.cache_flushes)
+        if self._cache_ready:
+            h, i, e, s = (int(v) for v in self.cache_stats.tolist())
+            out.update(hits=h, inserts=i, evictions=e, staged=s, steps=int(self.cache_step.item()))
+        return out
 
     def table(self, k: int) -> torch.Tensor:
         """[rows_k, D] view of table k (strided when the accumulator is interleaved; fp16 with emb_dtype="fp16").
@@ -681,7 +815,7 @@ class Engine:
             d.row_lo, d.row_n = int(sh["row_lo"]), int(sh["row_n"])
             if self.is_host[k]:      # the staged rows, read through the slot of every position
                 d.weight, d.indices = self.stage_w.data_ptr(), self._slot_ptr(sp, k)
-                d.rows, d.row_lo, d.row_n = self.stage_cap, 0, self.stage_cap
+                d.rows, d.row_lo, d.row_n = self._arena_rows, 0, self._arena_rows
             if route is not None:
                 d.out_off, d.out_stride = int(route[k][0]), int(route[k][1])
         return arr
@@ -698,7 +832,7 @@ class Engine:
                 d.use_dy_off, d.dy_off = 1, int(dy_off[k])
             d.weight = self.tables.data_ptr() + self._abase[k] * self.ldw * self.esize
             if self.is_host[k]:
-                d.weight, d.row_lo, d.row_n = self.stage_w.data_ptr(), 0, self.stage_cap
+                d.weight, d.row_lo, d.row_n = self.stage_w.data_ptr(), 0, self._arena_rows
             d.ld = self.ldw
             if self.f16:
                 d.weight_dtype = DTYPE_F16
@@ -727,7 +861,7 @@ class Engine:
             d.nnz = sp.indices[k].numel()
             d.rows = int(sh["rows"])
             if self.is_host[k]:
-                d.indices, d.rows = self._slot_ptr(sp, k), self.stage_cap
+                d.indices, d.rows = self._slot_ptr(sp, k), self._arena_rows
             d.pair_base = 0 if sp.include_last else base
             base += sp.indices[k].numel()
         total = sp.nnz_total if sp.include_last else base
@@ -753,7 +887,7 @@ class Engine:
         # host tables: stage the rows first (unless emb_link already staged this batch for its update)
         stage = bool(self.host) and not (self._staged is sp and self._staged_by_link)
         if stage:
-            self._stage_in(sp)
+            self._stage_in(sp, train=link)
         routed = out is None
         route = self.route_out if routed else [(k * stride_table, stride_sample) for k in range(self.T)]
         whole = [k for k in range(self.T) if int(self.shards[k]["nparts"]) == 1]
@@ -1594,6 +1728,7 @@ class GraphedTrainSteps:
         self.graph.replay()
         self.eng.n_launch += self.kernels_per_replay
         self.eng.opt_step += self.K
+        self.eng._cache_dirty = bool(self.eng.cache_rows)      # the steps may have inserted into the row cache
         return self.losses
 
 
@@ -1644,6 +1779,7 @@ class GraphedTrainStep:
         self.eng.n_launch += self.kernels_per_replay
         if self.train:
             self.eng.opt_step += 1
+            self.eng._cache_dirty = bool(self.eng.cache_rows)
         return self.out
 
 

@@ -557,6 +557,29 @@ typedef struct {
   int64_t capacity;     /* positions (and slots); every global position must be below it */
   int64_t ld;           /* floats per row; 0 = dim */
   int64_t head_col;     /* word of the row holding the list head (interleaved rows), or -1 */
+  /* Row cache (all zero: no cache, and every call behaves as described above).  With cache_rows = N > 0 the
+   * staging arrays weight / momentum / head / acc_ew hold N + capacity rows: slots [0, N) are the cache, kept
+   * across calls, and position p stages into slot N + p.  map[row] = slot + 1 then means a cache slot for 1..N
+   * and this step's staging slot above N; only the latter are cleared by write_back / release.  key[] stays
+   * [capacity], indexed by position.  The set of a row is splitmix64(row * 64 + table) mod (N / 32), 32 ways.
+   *   stage_in, training (forward_only = 0): a one-thread kernel, in place of the counter memset, advances *step
+   *                and resets count and num_sets; a resident row is a hit (its slot goes to slot_idx, its last use becomes *step); a missing row is
+   *                staged as above and threaded onto its set's list.
+   *   stage_in, forward_only = 1: hits are read from their slots, misses staged; no cache state changes.
+   *   write_back : per set with misses, the misses in ascending (table, row) order take the ways not used in this
+   *                step, empty ways first, then the oldest last use, ties to the lower way; a victim's row goes
+   *                to host memory and leaves the map; the miss moves into the slot.  Misses left over go home.
+   * stats: cumulative hits, inserts, evictions, staged (uncached) rows, each per distinct row of a training step. */
+  int64_t cache_rows;   /* N: a multiple of 32, N + capacity <= 2^31 - 2; 0 = no cache */
+  int64_t* cache_tag;   /* [N] row * 64 + table of a resident slot, -1 = empty */
+  int32_t* cache_used;  /* [N] training step of the slot's last use, 0 = empty */
+  int32_t* step;        /* one int32: the current training step, 0 before the first */
+  int32_t* set_head;    /* [N / 32] position + 1 of a set's first miss, zero between steps */
+  int32_t* set_next;    /* [capacity] */
+  int32_t* sets;        /* [N / 32] the sets with a miss in this step */
+  int32_t* num_sets;    /* one int32 */
+  int64_t* stats;       /* [4] hits, inserts, evictions, staged */
+  int64_t forward_only; /* 1: a pass without an update (see stage_in) */
 } dlrm_host_stage_t;
 
 int dlrm_b200_host_stage_in(const dlrm_host_table_t* tables /*[host]*/, int num_tables,
@@ -566,6 +589,10 @@ int dlrm_b200_host_write_back(const dlrm_host_table_t* tables /*[host]*/, int nu
                               const dlrm_host_stage_t* stage /*[host]*/, int dim, void* stream);
 int dlrm_b200_host_release(const dlrm_host_table_t* tables /*[host]*/, int num_tables,
                            const dlrm_host_stage_t* stage /*[host]*/, int dim, void* stream);
+/* Row cache: every resident row and its accumulators back to host memory (list head as zero), then its map entry,
+ * tag and last use cleared.  Counters and the step are kept.  Needs cache_rows > 0; no batch fields are read. */
+int dlrm_b200_host_cache_flush(const dlrm_host_table_t* tables /*[host]*/, int num_tables,
+                               const dlrm_host_stage_t* stage /*[host]*/, int dim, void* stream);
 /* Page-lock [ptr, ptr + bytes) of ordinary host memory as mapped memory (cudaHostRegister) and check that the
  * device address equals ptr; error (and nothing stays registered) otherwise.  Synchronous. */
 int dlrm_b200_host_register(void* ptr, int64_t bytes);
