@@ -70,7 +70,7 @@ class GemmTcDesc(C.Structure):
                 ("out_hi", C.c_void_p), ("out_lo", C.c_void_p), ("ld_out", C.c_int64),
                 ("outT_hi", C.c_void_p), ("outT_lo", C.c_void_p), ("ld_outT", C.c_int64),
                 ("out_col", C.c_void_p), ("col_index", C.c_int64), ("col_slab_stride", C.c_int64),
-                ("bias", C.c_void_p)]
+                ("bias", C.c_void_p), ("tile_m", C.c_int)]
 
 
 class DenseLayer(C.Structure):
@@ -144,7 +144,8 @@ def _declare(lib):
     lib.dlrm_b200_loss_fwd_bwd.argtypes = [vp, vp, vp, i64, i32, f32, i32, vp, vp, vp, vp]
     lib.dlrm_b200_dense_update.argtypes = [vp, vp, vp, i64, i32, f32, f32, vp]
     lib.dlrm_b200_gemm_tc_plan_create.argtypes = [C.POINTER(GemmTcDesc), C.POINTER(vp)]
-    lib.dlrm_b200_gemm_tc_plan_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
+    lib.dlrm_b200_gemm_tc_plan_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32),
+                                                C.POINTER(i32)]
     lib.dlrm_b200_gemm_tc_run.argtypes = [vp, vp]
     lib.dlrm_b200_emb_bwd_small_scratch_bytes.argtypes = [i64, i32, i64]
     lib.dlrm_b200_emb_bwd_small_update.argtypes = [C.POINTER(EmbBwdTable), i32, i32, i64, i32, i32, vp, C.POINTER(vp), i32,
@@ -228,9 +229,10 @@ class GemmTcPlan:
         check(lib().dlrm_b200_gemm_tc_plan_create(C.byref(d), C.byref(self.handle)), "gemm_tc_plan_create")
 
     def info(self):
-        a, b, c, e = C.c_int(), C.c_int(), C.c_int(), C.c_int()
-        check(lib().dlrm_b200_gemm_tc_plan_info(self.handle, C.byref(a), C.byref(b), C.byref(c), C.byref(e)))
-        return dict(tile_n=a.value, stages=b.value, splits=c.value, ctas=e.value)
+        a, b, c, e, m = C.c_int(), C.c_int(), C.c_int(), C.c_int(), C.c_int()
+        check(lib().dlrm_b200_gemm_tc_plan_info(self.handle, C.byref(a), C.byref(b), C.byref(c), C.byref(e),
+                                                C.byref(m)))
+        return dict(tile_n=a.value, stages=b.value, splits=c.value, ctas=e.value, tile_m=m.value)
 
     def run(self, stream):
         check(lib().dlrm_b200_gemm_tc_run(self.handle, stream), "gemm_tc_run")

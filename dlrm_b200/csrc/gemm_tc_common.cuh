@@ -113,13 +113,14 @@ template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 // wgmma shared-memory descriptor (sm_90): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), base offset 0
-// (every tile is 1024-byte aligned), layout SWIZZLE_128B=1 [62,64).
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// (every tile is 1024-byte aligned), layout [62,64): SWIZZLE_128B = 1, SWIZZLE_64B = 2.
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
+                                                   uint32_t layout = 1) {
   uint64_t d = 0;
   d |= (uint64_t)((addr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 62;
+  d |= (uint64_t)layout << 62;
   return d;
 }
 
@@ -133,45 +134,71 @@ __device__ __forceinline__ float apply_act_tc(float v, int act) {
 // ------------------------------------------------------------------------------------------ CTA layout
 // Warpgroup 0: warp 0 lane 0 is the TMA producer (warps 1-3 only exist so that the consumers are whole,
 // aligned warpgroups).  Warpgroups 1 and 2 are the consumers: consumer warpgroup w issues the wgmmas of
-// accumulator rows [64 w, 64 w + 64) of the 128 x BN tile, then all 8 consumer warps run the epilogue.
+// accumulator rows [BM/2 w, BM/2 w + BM/2) of the BM x BN tile, then all 8 consumer warps run the epilogue.
+// BM = 128: one m64 accumulator per consumer warpgroup, k blocks of 64 (128-byte rows, 128-byte swizzle).
+// BM = 256: two m64 accumulators per consumer warpgroup (128 fp32 registers per thread), k blocks of 32 so that
+// four x3 stages (48 KB each) fit the ring; K-major tiles then have 64-byte rows and use the 64-byte swizzle.
 constexpr int TC_EPI_WARPS = 8;
 constexpr int TC_THREADS = 128 + 32 * TC_EPI_WARPS;
 constexpr int TC_CONSUMER_WARP0 = 4;
 constexpr uint32_t TC_A_BYTES = TC_BM * TC_BK * 2;   // 16 KB; rows 64..127 start at +8 KB in both majornesses
 
+template <int BM>
+struct TcTile {
+  static constexpr int BK = BM == 256 ? 32 : TC_BK;
+  static constexpr int MT = BM / 128;                         // m64 accumulators per consumer warpgroup
+  static constexpr uint32_t A64_BYTES = 64 * BK * 2;          // 64 rows of A: the next 64 start here (both majornesses)
+  static constexpr uint32_t A_BYTES = BM * BK * 2;
+  static constexpr uint32_t KROW_BYTES = BK * 2;              // K-major row = swizzle span
+  static constexpr uint32_t LAYOUT = BK == 64 ? 1u : 2u;      // K-major descriptor layout: 128- / 64-byte swizzle
+  static constexpr uint32_t MN_BOX_BYTES = BK * 128;          // MN-major box: BK k rows of 64 mn
+};
+
 // Consumer main loop over k blocks [kb0, kb1) of one tile.  Every stage of the ring holds A_hi [A_lo] B_hi
-// [B_lo] (x3 adds the lo tiles), each 1024-byte aligned in the 128-byte swizzle TMA writes.  A stage is
-// released (one arrive per consumer warp) once the wgmmas that read it have retired; the wgmmas of the next
-// k block are already issued by then.  `stage` / `phase` carry the ring position across calls.
-//   K-major SW128 : rows of 128 B, 8-row groups 1024 B apart (SBO); a 16-wide k step = +32 B.
-//   MN-major SW128: [64 k rows][64 mn] boxes; 8-row k groups 1024 B apart (SBO), 64-wide mn blocks 8192 B
-//                   apart (LBO); a 16-deep k step = +2048 B.
-template <int BN, int TA, int TB>
-__device__ __forceinline__ void tc_mainloop_t(float (&d)[BN / 2], bool x3, uint32_t ring, uint32_t stage_bytes,
-                                              int stages, uint32_t bar_full, uint32_t bar_empty, int kb0, int kb1,
-                                              int& stage, uint32_t& phase, int wg, int lane) {
-  constexpr uint32_t B_BYTES = BN * TC_BK * 2;
-  constexpr uint32_t a_lbo = TA ? 8192u : 16u, b_lbo = TB ? 8192u : 16u;
+// [B_lo] (x3 adds the lo tiles), each 1024-byte aligned in the swizzle TMA writes.  A stage is released (one
+// arrive per consumer warp) once the wgmmas that read it have retired; the wgmmas of the next k block are already
+// issued by then.  `stage` / `phase` carry the ring position across calls.
+//   K-major SW128 / SW64 : rows of BK * 2 bytes, 8-row groups 8 rows apart (SBO); a 16-wide k step = +32 B.
+//   MN-major SW128       : [BK k rows][64 mn] boxes; 8-row k groups 1024 B apart (SBO), 64-wide mn blocks one box
+//                          apart (LBO); a 16-deep k step = +2048 B.
+// Every accumulator sees the same k16 sequence, and per k16 lo*hi, hi*lo, hi*hi, whatever BM and BK are: a
+// 256-row tile gives the bits of two 128-row tiles.
+template <int BM, int BN, int TA, int TB>
+__device__ __forceinline__ void tc_mainloop_t(float (&d)[TcTile<BM>::MT][BN / 2], bool x3, uint32_t ring,
+                                              uint32_t stage_bytes, int stages, uint32_t bar_full, uint32_t bar_empty,
+                                              int kb0, int kb1, int& stage, uint32_t& phase, int wg, int lane) {
+  using T = TcTile<BM>;
+  constexpr int MT = T::MT;
+  constexpr uint32_t B_BYTES = BN * T::BK * 2;
+  constexpr uint32_t a_lbo = TA ? T::MN_BOX_BYTES : 16u, b_lbo = TB ? T::MN_BOX_BYTES : 16u;
+  constexpr uint32_t a_sbo = TA ? 1024u : 8 * T::KROW_BYTES, b_sbo = TB ? 1024u : 8 * T::KROW_BYTES;
+  constexpr uint32_t a_lay = TA ? 1u : T::LAYOUT, b_lay = TB ? 1u : T::LAYOUT;
   int prev = -1;
   for (int kb = kb0; kb < kb1; ++kb) {
     mbar_wait(bar_full + 8 * stage, phase);
     __syncwarp();
-    const uint32_t sa_hi = ring + stage * stage_bytes + (uint32_t)wg * (TC_A_BYTES / 2);
-    const uint32_t sa_lo = sa_hi + TC_A_BYTES;
-    const uint32_t sb_hi = ring + stage * stage_bytes + (x3 ? 2u : 1u) * TC_A_BYTES;
+    const uint32_t sa_hi = ring + stage * stage_bytes + (uint32_t)(wg * MT) * T::A64_BYTES;
+    const uint32_t sa_lo = sa_hi + T::A_BYTES;
+    const uint32_t sb_hi = ring + stage * stage_bytes + (x3 ? 2u : 1u) * T::A_BYTES;
     const uint32_t sb_lo = sb_hi + B_BYTES;
     wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < TC_BK / 16; ++k) {
+    for (int k = 0; k < T::BK / 16; ++k) {
       const uint32_t a_off = TA ? k * 2048u : k * 32u;
       const uint32_t b_off = TB ? k * 2048u : k * 32u;
-      const uint64_t ah = make_smem_desc(sa_hi + a_off, a_lbo, 1024);
-      const uint64_t bh = make_smem_desc(sb_hi + b_off, b_lbo, 1024);
+      const uint64_t bh = make_smem_desc(sb_hi + b_off, b_lbo, b_sbo, b_lay);
       if (x3) {
-        wgmma_bf16<TA, TB>(d, make_smem_desc(sa_lo + a_off, a_lbo, 1024), bh);
-        wgmma_bf16<TA, TB>(d, ah, make_smem_desc(sb_lo + b_off, b_lbo, 1024));
+        const uint64_t bl = make_smem_desc(sb_lo + b_off, b_lbo, b_sbo, b_lay);
+#pragma unroll
+        for (int j = 0; j < MT; ++j)
+          wgmma_bf16<TA, TB>(d[j], make_smem_desc(sa_lo + j * T::A64_BYTES + a_off, a_lbo, a_sbo, a_lay), bh);
+#pragma unroll
+        for (int j = 0; j < MT; ++j)
+          wgmma_bf16<TA, TB>(d[j], make_smem_desc(sa_hi + j * T::A64_BYTES + a_off, a_lbo, a_sbo, a_lay), bl);
       }
-      wgmma_bf16<TA, TB>(d, ah, bh);
+#pragma unroll
+      for (int j = 0; j < MT; ++j)
+        wgmma_bf16<TA, TB>(d[j], make_smem_desc(sa_hi + j * T::A64_BYTES + a_off, a_lbo, a_sbo, a_lay), bh);
     }
     wgmma_commit();
     wgmma_wait<1>();                              // the previous k block's wgmmas have retired
@@ -183,34 +210,37 @@ __device__ __forceinline__ void tc_mainloop_t(float (&d)[BN / 2], bool x3, uint3
   if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
 }
 
-template <int BN>
-__device__ __forceinline__ void tc_mainloop(float (&d)[BN / 2], const TcArgs& g, uint32_t ring,
+template <int BM, int BN>
+__device__ __forceinline__ void tc_mainloop(float (&d)[TcTile<BM>::MT][BN / 2], const TcArgs& g, uint32_t ring,
                                             uint32_t stage_bytes, int stages, uint32_t bar_full, uint32_t bar_empty,
                                             int kb0, int kb1, int& stage, uint32_t& phase, int wg, int lane) {
 #pragma unroll
-  for (int j = 0; j < BN / 2; ++j) d[j] = 0.f;
+  for (int i = 0; i < TcTile<BM>::MT; ++i)
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) d[i][j] = 0.f;
   const bool x3 = g.x3 != 0;
   if (!g.a_mn && !g.b_mn)
-    tc_mainloop_t<BN, 0, 0>(d, x3, ring, stage_bytes, stages, bar_full, bar_empty, kb0, kb1, stage, phase, wg, lane);
+    tc_mainloop_t<BM, BN, 0, 0>(d, x3, ring, stage_bytes, stages, bar_full, bar_empty, kb0, kb1, stage, phase, wg, lane);
   else if (!g.a_mn)
-    tc_mainloop_t<BN, 0, 1>(d, x3, ring, stage_bytes, stages, bar_full, bar_empty, kb0, kb1, stage, phase, wg, lane);
+    tc_mainloop_t<BM, BN, 0, 1>(d, x3, ring, stage_bytes, stages, bar_full, bar_empty, kb0, kb1, stage, phase, wg, lane);
   else if (!g.b_mn)
-    tc_mainloop_t<BN, 1, 0>(d, x3, ring, stage_bytes, stages, bar_full, bar_empty, kb0, kb1, stage, phase, wg, lane);
+    tc_mainloop_t<BM, BN, 1, 0>(d, x3, ring, stage_bytes, stages, bar_full, bar_empty, kb0, kb1, stage, phase, wg, lane);
   else
-    tc_mainloop_t<BN, 1, 1>(d, x3, ring, stage_bytes, stages, bar_full, bar_empty, kb0, kb1, stage, phase, wg, lane);
+    tc_mainloop_t<BM, BN, 1, 1>(d, x3, ring, stage_bytes, stages, bar_full, bar_empty, kb0, kb1, stage, phase, wg, lane);
 }
 
 // ------------------------------------------------------------------------------------------ epilogue
-// The accumulator tile is staged in shared memory as fp32 [128][BN + 4] (the 4-float pad makes the epilogue's
+// The accumulator tile is staged in shared memory as fp32 [BM][BN + 4] (the 4-float pad makes the epilogue's
 // row-per-lane 16-byte reads conflict-free), then every consumer warp reads ONE ROW per lane, 32 consecutive
 // columns at a time.
 __host__ __device__ constexpr int tc_acc_ld(int bn) { return bn + 4; }
-__host__ __device__ constexpr int tc_acc_bytes(int bn) { return TC_BM * tc_acc_ld(bn) * 4; }
+__host__ __device__ constexpr int tc_acc_bytes(int bm, int bn) { return bm * tc_acc_ld(bn) * 4; }
 
-// consumer warp cw (0..7) stores its wgmma fragment: rows 16 cw + lane / 4 (+ 8), columns 8 j + 2 (lane % 4)
+// a consumer warp stores one m64 wgmma fragment of its warpgroup: rows row0 + lane / 4 (+ 8), columns
+// 8 j + 2 (lane % 4), where row0 = the fragment's first tile row + 16 x (the warp's rank in its warpgroup)
 template <int BN>
-__device__ __forceinline__ void tc_stage_acc(const float (&d)[BN / 2], float* acc, int cw, int lane) {
-  float* r0 = acc + (size_t)(16 * cw + (lane >> 2)) * tc_acc_ld(BN) + 2 * (lane & 3);
+__device__ __forceinline__ void tc_stage_acc(const float (&d)[BN / 2], float* acc, int row0, int lane) {
+  float* r0 = acc + (size_t)(row0 + (lane >> 2)) * tc_acc_ld(BN) + 2 * (lane & 3);
   float* r1 = r0 + 8 * tc_acc_ld(BN);
 #pragma unroll
   for (int j = 0; j < BN / 8; ++j) {
@@ -219,7 +249,7 @@ __device__ __forceinline__ void tc_stage_acc(const float (&d)[BN / 2], float* ac
   }
 }
 
-// Staged tile (128 rows x bn columns) -> global memory.
+// Staged tile (BM rows x bn columns) -> global memory.
 //
 // Storing straight from the row-per-lane layout would make each warp-wide 16-byte store hit 32 different rows
 // (32 half-written sectors per instruction).  Instead every 32 x 32 chunk is transposed through a per-warp
@@ -232,8 +262,8 @@ constexpr int TC_EPI_ROW_BF16 = 40;                // bf16 per staged bf16 row (
 constexpr int TC_EPI_WARP_BYTES = 32 * TC_EPI_ROW_BF16 * 2;  // 2560 B per epilogue warp (fp32: two 16-column passes)
 constexpr int TC_EPI_BYTES = TC_EPI_WARPS * TC_EPI_WARP_BYTES;
 // the accumulator is staged in the operand ring, idle once the last wgmma has retired
-__host__ __device__ constexpr size_t tc_ring_bytes(size_t ring, int bn) {
-  return ring > (size_t)tc_acc_bytes(bn) ? ring : (size_t)tc_acc_bytes(bn);
+__host__ __device__ constexpr size_t tc_ring_bytes(size_t ring, int bm, int bn) {
+  return ring > (size_t)tc_acc_bytes(bm, bn) ? ring : (size_t)tc_acc_bytes(bm, bn);
 }
 
 // 32 x 32 bf16 chunk, one row per thread in `mine` -> global rows [mrow0, mrow0 + 32) x columns [nb, nb + 32)
@@ -261,8 +291,8 @@ __device__ __forceinline__ void tc_epi_store_bf16(const __nv_bfloat16 (&mine)[32
   __syncwarp();
 }
 
-// This warp handles rows [32 quad, 32 quad + 32) of the tile and its 32-column chunks c0, c0 + cstep, ... (two
-// warps per 32-row block split the chunks of a tile between them).
+// This warp handles rows [32 quad, 32 quad + 32) of the tile and its 32-column chunks c0, c0 + cstep, ... (in a
+// 128-row tile two warps per 32-row block split the chunks between them; in a 256-row tile each warp has a block).
 __device__ __forceinline__ void tc_epilogue_tile(const TcArgs& g, int bn, int m0, int n0, int bz, const float* acc,
                                                  int quad, int lane, uint8_t* stage_warp, int c0, int cstep) {
   // Every field is copied into a register ONCE: `g` lives in kernel-parameter space and the mbarrier asm
@@ -441,7 +471,7 @@ __device__ __forceinline__ void tc_epilogue_tile(const TcArgs& g, int bn, int m0
 struct TcPlan {
   CUtensorMap tmAh, tmAl, tmBh, tmBl;
   TcArgs args;
-  int bn, stages, splits;
+  int bm, bn, stages, splits;
   size_t smem;
   dim3 grid;
 };

@@ -1393,7 +1393,10 @@ class Engine:
 
     def _tc_setup(self, B: int):
         dev, bf = self.device, torch.bfloat16
-        r8 = lambda v: (v + 7) // 8 * 8
+        # operand rows padded to 64 bf16 = 128 bytes: every row of a (hi, lo) operand then starts on a 128-byte line,
+        # so a TMA box row (64 or 128 bytes) covers whole 32-byte sectors (an ld of 1032 put every other 64-byte row
+        # across three sectors)
+        r64 = lambda v: (v + 63) // 64 * 64
         self.tc_B = B
         self.ntc = {"bot": self._tc_n("bot"), "top": self._tc_n("top")}
         self.tc_in, self.tc_gz, self.tc_W = {}, {}, {}
@@ -1426,7 +1429,7 @@ class Engine:
             ins, gzs, Ws = [], [], []
             for i in range(ntc):
                 K, N = ln[i], ln[i + 1]
-                Kp, Np = r8(K + 1), r8(N)
+                Kp, Np = r64(K + 1), r64(N)
                 h = torch.zeros((B, Kp), dtype=bf, device=dev)
                 l = torch.zeros((B, Kp), dtype=bf, device=dev)
                 h[:, K] = 1.0  # constant-1 column: bias folded into the GEMM

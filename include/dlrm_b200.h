@@ -393,10 +393,15 @@ typedef struct {
   void* outT_hi; void* outT_lo; int64_t ld_outT;
   float* out_col; int64_t col_index; int64_t col_slab_stride;
   const float* bias;  /* optional fp32 [N] added to the accumulator before act (nn.Linear bias in fp32) */
+  int tile_m;       /* rows per CTA tile: 0 = auto, 128 or 256.  256 needs a 128-wide tile and no split-K (refused
+                       otherwise); auto picks it for such plans when M >= 256, the grid keeps >= 120 CTAs and every
+                       K-major operand's ld is a multiple of 64 (128-byte rows).  Both heights give bit-identical
+                       results. */
 } dlrm_gemm_tc_desc_t;
 
 int dlrm_b200_gemm_tc_plan_create(const dlrm_gemm_tc_desc_t* desc /*[host]*/, void** plan);
-int dlrm_b200_gemm_tc_plan_info(void* plan, int* tile_n, int* stages, int* splits, int* ctas);
+/* tile_m (appended): the plan's rows per CTA tile, 128 or 256.  Any output pointer may be NULL. */
+int dlrm_b200_gemm_tc_plan_info(void* plan, int* tile_n, int* stages, int* splits, int* ctas, int* tile_m);
 int dlrm_b200_gemm_tc_run(void* plan, void* stream);
 int dlrm_b200_gemm_tc_plan_destroy(void* plan);
 
