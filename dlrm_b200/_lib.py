@@ -101,6 +101,8 @@ SYMBOLS = [
     "dlrm_b200_decode_records", "dlrm_b200_gather_records", "dlrm_b200_ingest_records",
     "dlrm_b200_host_stage_in", "dlrm_b200_host_write_back", "dlrm_b200_host_release", "dlrm_b200_host_register",
     "dlrm_b200_host_unregister", "dlrm_b200_host_cache_flush",
+    "dlrm_b200_emb_bwd_update_lr_dev", "dlrm_b200_emb_bwd_small_update_lr_dev", "dlrm_b200_dense_update_lr_dev",
+    "dlrm_b200_dense_update_pack_lr_dev",
 ]
 
 
@@ -167,6 +169,12 @@ def _declare(lib):
     lib.dlrm_b200_host_cache_flush.argtypes = [C.POINTER(HostTable), i32, C.POINTER(HostStage), i32, vp]
     lib.dlrm_b200_host_register.argtypes = [vp, i64]
     lib.dlrm_b200_host_unregister.argtypes = [vp]
+    lib.dlrm_b200_emb_bwd_update_lr_dev.argtypes = [C.POINTER(EmbBwdTable), i32, i32, i64, i32, i32, vp, vp,
+                                                    i64, i64, i32, f32, vp, f32, C.POINTER(EmbDedup), vp]
+    lib.dlrm_b200_emb_bwd_small_update_lr_dev.argtypes = [C.POINTER(EmbBwdTable), i32, i32, i64, i32, i32, vp,
+                                                          C.POINTER(vp), i32, i64, i64, i32, f32, vp, f32, vp, i64, vp]
+    lib.dlrm_b200_dense_update_lr_dev.argtypes = [vp, vp, vp, i64, i32, f32, vp, f32, vp]
+    lib.dlrm_b200_dense_update_pack_lr_dev.argtypes = [C.POINTER(DenseLayer), i32, i32, f32, vp, f32, vp]
     for name in SYMBOLS:
         fn = getattr(lib, name)
         if name in ("dlrm_b200_head_scratch_bytes", "dlrm_b200_emb_bwd_small_scratch_bytes"):

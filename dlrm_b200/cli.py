@@ -105,6 +105,8 @@ def build_parser():
     # dlrm_b200 addition: rows of the host tables kept in HBM between steps ("" none, "auto": the device memory left
     # free beyond the reserve of --emb-host-tables=auto, or a row count)
     p.add_argument("--emb-host-cache", type=str, default="")
+    # dlrm_b200 addition: full-size batches train (and test) by replaying a captured CUDA graph (graph_steps.py)
+    p.add_argument("--cuda-graph-steps", action="store_true", default=False)
     return p
 
 
@@ -226,6 +228,15 @@ def run(argv=None):
     if args.mlperf_logging and int(os.environ.get("WORLD_SIZE", "1")) > 1:
         sys.exit("ERROR: --mlperf-logging runs on one GPU (the device-side test metrics of a sharded run, which would "
                  "need every rank's scores gathered, are not supported)")
+    if args.cuda_graph_steps:
+        if args.emb_dtype == "fp16":
+            sys.exit("ERROR: --cuda-graph-steps needs --emb-dtype=fp32 (the stochastic-rounding keys of fp16 tables "
+                     "change every step, a captured step would replay one step's)")
+        if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+            sys.exit("ERROR: --cuda-graph-steps runs on one GPU (sharded runs are not captured)")
+        if args.data_generation in ("random", "synthetic"):
+            sys.exit("ERROR: --cuda-graph-steps needs --data-generation=dataset (the random generator de-duplicates "
+                     "each bag, so the number of indices changes from batch to batch)")
     if args.quantize_emb_with_bit in [4, 8] or args.quantize_mlp_with_bit != 32:
         sys.exit("ERROR: 4 and 8-bit quantization on GPU is not supported")
     if not torch.cuda.is_available():
@@ -496,6 +507,12 @@ def run(argv=None):
         else:
             print("Testing state: accuracy = {:3.3f} %".format(ld_acc_test * 100))
 
+    graphs = None
+    if args.cuda_graph_steps:     # captured after --load-model: the graphs run on the restored state
+        from .graph_steps import GraphSteps
+
+        test_B = args.test_mini_batch_size if (args.inference_only or args.test_freq > 0) else None
+        graphs = GraphSteps(dlrm, optimizer, args.mini_batch_size, test_B, m_den, args.optimizer)
     score_keys = None
 
     def inference(best_acc, best_auc=0.0):
@@ -515,15 +532,16 @@ def run(argv=None):
             if nbatches > 0 and i >= nbatches:
                 break
             X_t, lS_o_t, lS_i_t, T_t = test_batch(i)
+            Z_g = graphs.forward(X_t, lS_o_t, lS_i_t) if graphs is not None else None
             if args.mlperf_logging:
                 with torch.no_grad():
-                    score_keys.add(dlrm(X_t.to(device), lS_o_t, lS_i_t), T_t.to(device))
+                    score_keys.add(Z_g if Z_g is not None else dlrm(X_t.to(device), lS_o_t, lS_i_t), T_t.to(device))
                 continue
             if world > 1 and X_t.size(0) % world != 0:
                 print("Warning: Skiping the batch %d with size %d" % (i, X_t.size(0)))
                 continue
             with torch.no_grad():
-                Z_t = dlrm(X_t.to(device), lS_o_t, lS_i_t)
+                Z_t = Z_g if Z_g is not None else dlrm(X_t.to(device), lS_o_t, lS_i_t)
             if world > 1:
                 import torch.distributed as tdist
 
@@ -591,27 +609,32 @@ def run(argv=None):
                     continue
                 torch.cuda.synchronize()
                 t1 = time.time()
-                Z = dlrm(X.to(device), lS_o, lS_i)
-                if world > 1:                               # loss on this rank's batch slice (:1584-1586)
-                    nloc = X.size(0) // world
-                    T = T[rank * nloc:(rank + 1) * nloc]
-                Td = T.to(device)
-                if args.loss_function == "wbce":
-                    ws = dlrm.loss_ws.to(device)[Td.view(-1).long()].view_as(Td).float()
-                    E = (ws * dlrm.loss_fn(Z, Td)).mean()
+                # --cuda-graph-steps: a full-size batch is one replay of the captured step (None: eager step below)
+                E = graphs.train(X, lS_o, lS_i, T) if graphs is not None else None
+                if E is not None:
+                    L = E[0].cpu().numpy()
                 else:
-                    E = dlrm.loss_fn(Z, Td)
-                L = E.detach().cpu().numpy()
-                if world > 1 and os.environ.get("DLRM_CLI_GLOBAL_LOSS") == "1":
-                    # the reference prints rank 0's slice loss; the mean over the ranks is the single-process loss
-                    import torch.distributed as tdist
+                    Z = dlrm(X.to(device), lS_o, lS_i)
+                    if world > 1:                               # loss on this rank's batch slice (:1584-1586)
+                        nloc = X.size(0) // world
+                        T = T[rank * nloc:(rank + 1) * nloc]
+                    Td = T.to(device)
+                    if args.loss_function == "wbce":
+                        ws = dlrm.loss_ws.to(device)[Td.view(-1).long()].view_as(Td).float()
+                        E = (ws * dlrm.loss_fn(Z, Td)).mean()
+                    else:
+                        E = dlrm.loss_fn(Z, Td)
+                    L = E.detach().cpu().numpy()
+                    if world > 1 and os.environ.get("DLRM_CLI_GLOBAL_LOSS") == "1":
+                        # the reference prints rank 0's slice loss; the mean over the ranks is the single-process loss
+                        import torch.distributed as tdist
 
-                    Lg = E.detach().clone()
-                    tdist.all_reduce(Lg, op=tdist.ReduceOp.AVG)
-                    L = Lg.cpu().numpy()
-                optimizer.zero_grad()
-                E.backward()
-                optimizer.step()
+                        Lg = E.detach().clone()
+                        tdist.all_reduce(Lg, op=tdist.ReduceOp.AVG)
+                        L = Lg.cpu().numpy()
+                    optimizer.zero_grad()
+                    E.backward()
+                    optimizer.step()
                 lr_scheduler.step()
                 torch.cuda.synchronize()
                 total_time += time.time() - t1
@@ -649,6 +672,8 @@ def run(argv=None):
                               + " reached, stop training")
                         stop = True
                         break
+    if graphs is not None:
+        print(graphs.report())
     if days:                                                # the inflate threads end with the run
         train_data.close()
         test_data.close()

@@ -195,7 +195,11 @@ struct EmbBwdParams {
   // fp16 tables: stochastic-rounding key of table k for this step (kept out of EmbBwdTable, so that the fp32
   // kernels see the parameter layout they always had)
   unsigned long long round_key[DLRM_B200_MAX_TABLES_PER_CALL];
+  // learning rate in device memory (CUDA-graph steps whose rate changes between replays); NULL: lr above
+  const float* lr_dev;
 };
+
+__device__ __forceinline__ float step_lr(const EmbBwdParams& P) { return P.lr_dev ? *P.lr_dev : P.lr; }
 
 __device__ __forceinline__ const float* dy_row(const EmbBwdParams& P, long long bag) {
   if (P.peer_batch > 0) {
@@ -516,7 +520,7 @@ __global__ void __launch_bounds__(256, NV == 1 ? (EW ? 2 : 3) : 1) emb_update_ke
         }
         if constexpr (EW) {
           (void)m_old;
-          const float nlr = -P.lr;
+          const float nlr = -step_lr(P);
           float* srow = tb.mom + r * tb.mom_stride;
 #pragma unroll
           for (int v = 0; v < NV; ++v)
@@ -537,7 +541,7 @@ __global__ void __launch_bounds__(256, NV == 1 ? (EW ? 2 : 3) : 1) emb_update_ke
           sq = warp_sum(sq);
           const float m_new = m_old + sq * inv_d;
           const float stdv = sqrtf(m_new) + P.eps;
-          const float nlr = -P.lr;
+          const float nlr = -step_lr(P);
 #pragma unroll
           for (int v = 0; v < NV; ++v)
             if (col_ok[v]) {
@@ -547,7 +551,7 @@ __global__ void __launch_bounds__(256, NV == 1 ? (EW ? 2 : 3) : 1) emb_update_ke
             }
           if (lane == 0) tb.mom[r * tb.mom_stride] = m_new;
         } else {
-          const float nlr = -P.lr;
+          const float nlr = -step_lr(P);
 #pragma unroll
           for (int v = 0; v < NV; ++v)
             if (col_ok[v]) {
@@ -667,7 +671,7 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
   const long long warp0 = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const long long wstep = (long long)gridDim.x * (blockDim.x >> 5) * 32;
   const float inv_d = 1.0f / (float)D;
-  const float nlr = -P.lr;
+  const float nlr = -step_lr(P);
   const bool adagrad = !EW && P.optimizer == DLRM_OPT_RWSADAGRAD;    // row-wise
   const int dbg = P.debug;
 
@@ -919,7 +923,7 @@ static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, i
                            int idx_bytes, int include_last, const int32_t* next, const float* dY,
                            int64_t dy_stride_sample, int64_t dy_stride_table, int optimizer, float lr,
                            float eps, void* stream, const float* const* peer_dY, int world,
-                           int64_t batch_local, const dlrm_emb_dedup_t* dedup) {
+                           int64_t batch_local, const dlrm_emb_dedup_t* dedup, const float* lr_dev = nullptr) {
   using namespace dlrm;
   EmbBwdParams P{};
   if (int rc = fill_params(P, tables, num_tables, "emb_bwd_update")) return rc;
@@ -977,6 +981,7 @@ static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, i
   P.include_last = include_last;
   P.optimizer = optimizer;
   P.lr = lr;
+  P.lr_dev = lr_dev;
   P.eps = eps;
   P.debug = get_tunable(TUNE_UPD_DEBUG);
   const int block = 256;
@@ -1069,6 +1074,16 @@ extern "C" int dlrm_b200_emb_bwd_update(const dlrm_emb_bwd_table_t* tables, int 
                                         void* stream) {
   return emb_update_impl(tables, num_tables, dim, batch, idx_bytes, include_last, next, dY, dy_stride_sample,
                          dy_stride_table, optimizer, lr, eps, stream, nullptr, 0, 0, dedup);
+}
+
+extern "C" int dlrm_b200_emb_bwd_update_lr_dev(const dlrm_emb_bwd_table_t* tables, int num_tables, int dim,
+                                               int64_t batch, int idx_bytes, int include_last,
+                                               const int32_t* next, const float* dY,
+                                               int64_t dy_stride_sample, int64_t dy_stride_table,
+                                               int optimizer, float lr, const float* lr_dev, float eps,
+                                               const dlrm_emb_dedup_t* dedup, void* stream) {
+  return emb_update_impl(tables, num_tables, dim, batch, idx_bytes, include_last, next, dY, dy_stride_sample,
+                         dy_stride_table, optimizer, lr, eps, stream, nullptr, 0, 0, dedup, lr_dev);
 }
 
 extern "C" int dlrm_b200_emb_bwd_classify(const dlrm_emb_bwd_table_t* tables, int num_tables, int64_t batch,

@@ -48,6 +48,7 @@ struct SmallParams {
   float* partial;       // [chunks][total small rows][dim]
   int total_rows, chunks;
   unsigned long long round_key[SMALL_MAX_TABLES];   // fp16: stochastic-rounding key of table k for this step
+  const float* lr_dev;  // learning rate in device memory; NULL: lr above
 };
 
 __device__ __forceinline__ const float* small_dy_row(const SmallParams& P, long long bag) {
@@ -159,7 +160,7 @@ __global__ void __launch_bounds__(256) emb_small_apply_kernel(const __grid_const
       }
   }
   wt* wrow = static_cast<wt*>(tb.w) + (long long)r * tb.ld + lane * 4;
-  const float nlr = -P.lr;
+  const float nlr = -(P.lr_dev ? *P.lr_dev : P.lr);
   unsigned long long rkey = 0;
   if constexpr (is_f16<wt>::value) rkey = sr_row_key(P.round_key[k], r + tb.row_lo);
   // untouched row (or an all-zero gradient): nothing changes.  Tested on g itself, not on its sum of squares: a row
@@ -223,11 +224,10 @@ extern "C" int64_t dlrm_b200_emb_bwd_small_scratch_bytes(int64_t total_small_row
   return chunks * total_small_rows * dim * 4;
 }
 
-extern "C" int dlrm_b200_emb_bwd_small_update(const dlrm_emb_bwd_table_t* tables, int num_tables, int dim,
-                                              int64_t batch, int idx_bytes, int include_last, const float* dY,
-                                              const float* const* peer_dY, int world, int64_t batch_local,
-                                              int64_t dy_stride_sample, int optimizer, float lr, float eps,
-                                              float* scratch, int64_t scratch_bytes, void* stream) {
+static int small_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, int dim, int64_t batch,
+                             int idx_bytes, int include_last, const float* dY, const float* const* peer_dY, int world,
+                             int64_t batch_local, int64_t dy_stride_sample, int optimizer, float lr,
+                             const float* lr_dev, float eps, float* scratch, int64_t scratch_bytes, void* stream) {
   using namespace dlrm;
   if (num_tables == 0 || batch == 0) return 0;
   if (num_tables < 0 || num_tables > SMALL_MAX_TABLES) return set_error("emb_bwd_small_update: num_tables=%d (max %d)", num_tables, SMALL_MAX_TABLES);
@@ -285,7 +285,7 @@ extern "C" int dlrm_b200_emb_bwd_small_update(const dlrm_emb_bwd_table_t* tables
     }
     P.peer_batch = batch_local;
   }
-  P.batch = batch; P.dim = dim; P.include_last = include_last; P.optimizer = optimizer; P.lr = lr; P.eps = eps;
+  P.batch = batch; P.dim = dim; P.include_last = include_last; P.optimizer = optimizer; P.lr = lr; P.lr_dev = lr_dev; P.eps = eps;
   P.partial = scratch; P.total_rows = total_rows; P.chunks = chunks;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int nv = (dim + 127) / 128;
@@ -313,4 +313,23 @@ extern "C" int dlrm_b200_emb_bwd_small_update(const dlrm_emb_bwd_table_t* tables
   if (nv == 2) SMALL_LAUNCH(2, int);
   SMALL_LAUNCH(4, int);
 #undef SMALL_LAUNCH
+}
+
+extern "C" int dlrm_b200_emb_bwd_small_update(const dlrm_emb_bwd_table_t* tables, int num_tables, int dim,
+                                              int64_t batch, int idx_bytes, int include_last, const float* dY,
+                                              const float* const* peer_dY, int world, int64_t batch_local,
+                                              int64_t dy_stride_sample, int optimizer, float lr, float eps,
+                                              float* scratch, int64_t scratch_bytes, void* stream) {
+  return small_update_impl(tables, num_tables, dim, batch, idx_bytes, include_last, dY, peer_dY, world, batch_local,
+                           dy_stride_sample, optimizer, lr, nullptr, eps, scratch, scratch_bytes, stream);
+}
+
+extern "C" int dlrm_b200_emb_bwd_small_update_lr_dev(const dlrm_emb_bwd_table_t* tables, int num_tables, int dim,
+                                                     int64_t batch, int idx_bytes, int include_last, const float* dY,
+                                                     const float* const* peer_dY, int world, int64_t batch_local,
+                                                     int64_t dy_stride_sample, int optimizer, float lr,
+                                                     const float* lr_dev, float eps, float* scratch,
+                                                     int64_t scratch_bytes, void* stream) {
+  return small_update_impl(tables, num_tables, dim, batch, idx_bytes, include_last, dY, peer_dY, world, batch_local,
+                           dy_stride_sample, optimizer, lr, lr_dev, eps, scratch, scratch_bytes, stream);
 }

@@ -58,9 +58,11 @@ __global__ void __launch_bounds__(1024) loss_kernel(const float* __restrict__ p,
 __global__ void __launch_bounds__(256) dense_update_kernel(float* __restrict__ p,
                                                            const float* __restrict__ g,
                                                            float* __restrict__ s, long long n,
-                                                           int opt, float lr, float eps) {
+                                                           int opt, float lr, const float* lr_dev,
+                                                           float eps) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
+  if (lr_dev) lr = *lr_dev;
   const float gi = g[i];
   if (opt == DLRM_OPT_RWSADAGRAD) {
     const float si = fmaf(gi, gi, s[i]);
@@ -113,8 +115,8 @@ extern "C" int dlrm_b200_loss_fwd_bwd(const float* p, const float* target, const
   return 0;
 }
 
-extern "C" int dlrm_b200_dense_update(float* param, const float* grad, float* state, int64_t n,
-                                      int optimizer, float lr, float eps, void* stream) {
+static int dense_update_impl(float* param, const float* grad, float* state, int64_t n, int optimizer, float lr,
+                             const float* lr_dev, float eps, void* stream) {
   using namespace dlrm;
   if (n == 0) return 0;
   if (optimizer == DLRM_OPT_ADAGRAD) optimizer = DLRM_OPT_RWSADAGRAD;   // the dense branches are the same algorithm
@@ -123,7 +125,17 @@ extern "C" int dlrm_b200_dense_update(float* param, const float* grad, float* st
   if (!param || !grad || (optimizer == DLRM_OPT_RWSADAGRAD && !state))
     return set_error("dense_update: NULL pointer");
   dense_update_kernel<<<(unsigned)((n + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      param, grad, state, n, optimizer, lr, eps);
+      param, grad, state, n, optimizer, lr, lr_dev, eps);
   DLRM_CHECK_LAUNCH("dense_update_kernel");
   return 0;
+}
+
+extern "C" int dlrm_b200_dense_update(float* param, const float* grad, float* state, int64_t n,
+                                      int optimizer, float lr, float eps, void* stream) {
+  return dense_update_impl(param, grad, state, n, optimizer, lr, nullptr, eps, stream);
+}
+
+extern "C" int dlrm_b200_dense_update_lr_dev(float* param, const float* grad, float* state, int64_t n,
+                                             int optimizer, float lr, const float* lr_dev, float eps, void* stream) {
+  return dense_update_impl(param, grad, state, n, optimizer, lr, lr_dev, eps, stream);
 }

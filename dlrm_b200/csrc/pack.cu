@@ -38,6 +38,7 @@ struct DenseLayers {
   int num_layers;
   int optimizer;
   float lr, eps;
+  const float* lr_dev;         // learning rate in device memory; NULL: lr above
 };
 
 __global__ void __launch_bounds__(256) dense_update_pack_kernel(const __grid_constant__ DenseLayers P) {
@@ -67,13 +68,14 @@ __global__ void __launch_bounds__(256) dense_update_pack_kernel(const __grid_con
     }
     float* pp = is_b ? L.b : L.W;
     float p = pp[o];
+    const float lr = P.lr_dev ? *P.lr_dev : P.lr;
     if (P.optimizer == DLRM_OPT_RWSADAGRAD) {
       float* sp = is_b ? L.sb : L.sW;
       const float s2 = fmaf(g, g, sp[o]);
       sp[o] = s2;
-      p = fmaf(-P.lr, g / (sqrtf(s2) + P.eps), p);
+      p = fmaf(-lr, g / (sqrtf(s2) + P.eps), p);
     } else if (P.optimizer == DLRM_OPT_SGD) {
-      p = fmaf(-P.lr, g, p);
+      p = fmaf(-lr, g, p);
     }  // optimizer < 0: pack only
     pp[o] = p;
     if (L.hi) {
@@ -99,8 +101,8 @@ extern "C" int dlrm_b200_split_bf16(const float* X, int64_t ldx, int64_t M, int6
   return 0;
 }
 
-extern "C" int dlrm_b200_dense_update_pack(const dlrm_dense_layer_t* layers, int num_layers, int optimizer,
-                                           float lr, float eps, void* stream) {
+static int dense_update_pack_impl(const dlrm_dense_layer_t* layers, int num_layers, int optimizer, float lr,
+                                  const float* lr_dev, float eps, void* stream) {
   using namespace dlrm;
   if (num_layers <= 0) return 0;
   if (num_layers > 16) return set_error("dense_update_pack: at most 16 layers per call (got %d)", num_layers);
@@ -128,8 +130,18 @@ extern "C" int dlrm_b200_dense_update_pack(const dlrm_dense_layer_t* layers, int
   if (ctas >= (1ll << 31)) return set_error("dense_update_pack: too many parameters");
   for (int i = num_layers; i <= 16; ++i) P.cta_begin[i] = (int)ctas;
   P.num_layers = num_layers;
-  P.optimizer = optimizer; P.lr = lr; P.eps = eps;
+  P.optimizer = optimizer; P.lr = lr; P.eps = eps; P.lr_dev = lr_dev;
   (void)launch_chain(dense_update_pack_kernel, dim3((unsigned)ctas), dim3(256), 0, static_cast<cudaStream_t>(stream), P);
   DLRM_CHECK_LAUNCH("dense_update_pack_kernel");
   return 0;
+}
+
+extern "C" int dlrm_b200_dense_update_pack(const dlrm_dense_layer_t* layers, int num_layers, int optimizer,
+                                           float lr, float eps, void* stream) {
+  return dense_update_pack_impl(layers, num_layers, optimizer, lr, nullptr, eps, stream);
+}
+
+extern "C" int dlrm_b200_dense_update_pack_lr_dev(const dlrm_dense_layer_t* layers, int num_layers, int optimizer,
+                                                  float lr, const float* lr_dev, float eps, void* stream) {
+  return dense_update_pack_impl(layers, num_layers, optimizer, lr, lr_dev, eps, stream);
 }

@@ -151,6 +151,7 @@ class Engine:
         self.tc_x3 = 1 if gemm == "tc" else 0
         self.tc_B = -1                       # batch size the wgmma plans were built for
         self._pack_dirty = True
+        self._tc_kept = {}                   # B -> wgmma state a captured CUDA graph runs on (kept, see _tc_keep)
         if self.ln_bot[-1] != self.D:
             raise ValueError("bottom MLP output %d != sparse feature size %d" % (self.ln_bot[-1], self.D))
         if op == "dot":
@@ -239,6 +240,10 @@ class Engine:
         if loss_ws is not None:
             self.loss_ws = torch.as_tensor(loss_ws, dtype=torch.float32, device=dev)
         self.opt_step = 0
+        # While set (a CUDA graph being captured with GraphedTrainStep(device_lr=True)), the optimizer kernels read the
+        # learning rate from this device float instead of taking it by value; `lr_scalar` is the engine's one.
+        self.lr_dev: Optional[torch.Tensor] = None
+        self.lr_scalar: Optional[torch.Tensor] = None
         self._marks = None      # phase timeline (bench.py --phases): list of (name, stream tag, CUDA event)
         # hooks replaced by dlrm_b200.dist for table-wise sharded runs
         self.gather_fn = None       # (sp, link) -> fills Tbuf[:, 1:, :] for the LOCAL batch
@@ -1022,6 +1027,10 @@ class Engine:
             self._alloc_activations(B)
         if train and self.T:
             self._ensure_link(sp.nnz_total if sp.include_last else sum(int(i.numel()) for i in sp.indices))
+        small = [k for k in range(self.T) if self.is_small(k)]
+        if train and small:
+            self._ensure_small_scratch(max(sum(self.ln_emb[k] for k in small[c0:c0 + 32])
+                                           for c0 in range(0, len(small), 32)), B)
         if self.host:
             self._ensure_stage(max(int(sp.nnz_total if sp.include_last else sum(int(i.numel()) for i in sp.indices)),
                                    1), sp.idx_bytes)
@@ -1094,14 +1103,16 @@ class Engine:
                 if optimizer == "adagrad":
                     self._point_at_acc_ew(desc, ks)
                 rows = sum(self.ln_emb[k] for k in ks)
-                need = int(self.lib.dlrm_b200_emb_bwd_small_scratch_bytes(rows, self.D, sp.batch))
-                if getattr(self, "small_scratch", None) is None or self.small_scratch.numel() * 4 < need:
-                    self.small_scratch = torch.zeros(max(need // 4, 1), dtype=torch.float32, device=self.device)
-                _lib.check(self.lib.dlrm_b200_emb_bwd_small_update(
-                    desc, len(ks), self.D, sp.batch, sp.idx_bytes, int(sp.include_last), base,
-                    peer[0] if peer is not None else None, peer[1] if peer is not None else 0,
-                    peer[2] if peer is not None else 0, ss, _OPT[optimizer], lr, eps, self.small_scratch.data_ptr(),
-                    self.small_scratch.numel() * 4, _stream()), "emb_bwd_small_update")
+                self._ensure_small_scratch(rows, sp.batch)
+                args = (desc, len(ks), self.D, sp.batch, sp.idx_bytes, int(sp.include_last), base,
+                        peer[0] if peer is not None else None, peer[1] if peer is not None else 0,
+                        peer[2] if peer is not None else 0, ss, _OPT[optimizer], lr)
+                tail = (eps, self.small_scratch.data_ptr(), self.small_scratch.numel() * 4, _stream())
+                if self.lr_dev is None:
+                    _lib.check(self.lib.dlrm_b200_emb_bwd_small_update(*args, *tail), "emb_bwd_small_update")
+                else:
+                    _lib.check(self.lib.dlrm_b200_emb_bwd_small_update_lr_dev(*args, self.lr_dev.data_ptr(), *tail),
+                               "emb_bwd_small_update_lr_dev")
                 self.n_launch += 2
         for c0 in range(0, len(big), _lib.MAX_TABLES):
             ks = big[c0:c0 + _lib.MAX_TABLES]
@@ -1110,19 +1121,32 @@ class Engine:
                 self._point_at_acc_ew(desc, ks)
             dd = C.byref(self.dedup) if self._filtered else None
             if peer is not None:
+                if self.lr_dev is not None:
+                    raise RuntimeError("a device learning rate is not supported on sharded runs")
                 _lib.check(self.lib.dlrm_b200_emb_bwd_update_p2p(desc, len(ks), self.D, sp.batch, sp.idx_bytes,
                                                                  int(sp.include_last), self.link.data_ptr(), peer[0],
                                                                  peer[1], peer[2], ss, 0, _OPT[optimizer], lr, eps, dd,
                                                                  _stream()), "emb_bwd_update_p2p")
-            else:
+            elif self.lr_dev is None:
                 _lib.check(self.lib.dlrm_b200_emb_bwd_update(desc, len(ks), self.D, sp.batch, sp.idx_bytes,
                                                              int(sp.include_last), self.link.data_ptr(), base, ss, 0,
                                                              _OPT[optimizer], lr, eps, dd, _stream()), "emb_bwd_update")
+            else:
+                _lib.check(self.lib.dlrm_b200_emb_bwd_update_lr_dev(desc, len(ks), self.D, sp.batch, sp.idx_bytes,
+                                                                    int(sp.include_last), self.link.data_ptr(), base,
+                                                                    ss, 0, _OPT[optimizer], lr,
+                                                                    self.lr_dev.data_ptr(), eps, dd, _stream()),
+                           "emb_bwd_update_lr_dev")
             self.n_launch += 1
         if self.host:
             self._stage_out(True)       # same stream as the update: the rows go home before anything reads them
         if side:
             self._join(self.s_small)
+
+    def _ensure_small_scratch(self, rows: int, batch: int):
+        need = int(self.lib.dlrm_b200_emb_bwd_small_scratch_bytes(rows, self.D, batch))
+        if getattr(self, "small_scratch", None) is None or self.small_scratch.numel() * 4 < need:
+            self.small_scratch = torch.zeros(max(need // 4, 1), dtype=torch.float32, device=self.device)
 
     def mlp_backward(self, which: str, x_in: torch.Tensor, ldx: int, in_act: int, B: int,
                      acts: List[torch.Tensor], act_ld: List[int], gz: List[torch.Tensor],
@@ -1277,9 +1301,15 @@ class Engine:
         return self.Rbuf[:B, :self.num_int]
 
     def dense_step(self, optimizer: str, lr: float, eps: float = 1e-10):
-        _lib.check(self.lib.dlrm_b200_dense_update(self.dense.data_ptr(), self.dense_grad.data_ptr(),
-                                                   _ptr(self.dense_state), self.dense_numel, _OPT[optimizer],
-                                                   lr, eps, _stream()), "dense_update")
+        if self.lr_dev is None:
+            _lib.check(self.lib.dlrm_b200_dense_update(self.dense.data_ptr(), self.dense_grad.data_ptr(),
+                                                       _ptr(self.dense_state), self.dense_numel, _OPT[optimizer],
+                                                       lr, eps, _stream()), "dense_update")
+        else:
+            _lib.check(self.lib.dlrm_b200_dense_update_lr_dev(self.dense.data_ptr(), self.dense_grad.data_ptr(),
+                                                              _ptr(self.dense_state), self.dense_numel,
+                                                              _OPT[optimizer], lr, self.lr_dev.data_ptr(), eps,
+                                                              _stream()), "dense_update_lr_dev")
         self.n_launch += 1
 
     def train_step(self, X: torch.Tensor, sp: SparseInput, target: torch.Tensor, lr: float,
@@ -1391,7 +1421,24 @@ class Engine:
             return 0
         return n
 
+    def _tc_keep(self):
+        """Keep the current wgmma state (operand buffers, weight copies, plans) alive for its batch size: a captured
+        CUDA graph runs on it, so a step at another batch size must not release it, and _tc_setup restores it when
+        that batch size comes back."""
+        self._tc_kept[self.tc_B] = (self.ntc, self.tc_in, self.tc_gz, self.tc_W, self.tc_plans, self.tc_splits,
+                                    self._dense_off, self.dense_grad)
+
     def _tc_setup(self, B: int):
+        kept = self._tc_kept.get(B)
+        if kept is not None:
+            if kept[7] is not self.dense_grad:
+                raise RuntimeError("the weight-gradient arena was reallocated after a CUDA graph was captured at "
+                                   "batch %d: prepare the largest batch before capturing" % B)
+            (self.ntc, self.tc_in, self.tc_gz, self.tc_W, self.tc_plans, self.tc_splits,
+             self._dense_off, _) = kept
+            self.tc_B = B
+            self._pack_dirty = True       # this state's weight copies missed the updates made at other batch sizes
+            return
         dev, bf = self.device, torch.bfloat16
         # operand rows padded to 64 bf16 = 128 bytes: every row of a (hi, lo) operand then starts on a 128-byte line,
         # so a TMA box row (64 or 128 bytes) covers whole 32-byte sectors (an ld of 1032 put every other 64-byte row
@@ -1524,8 +1571,13 @@ class Engine:
         for c0 in range(0, len(layers), 16):
             chunk = layers[c0:c0 + 16]
             arr = (_lib.DenseLayer * len(chunk))(*chunk)
-            _lib.check(self.lib.dlrm_b200_dense_update_pack(arr, len(chunk), opt_code, lr, eps, _stream()),
-                       "dense_update_pack")
+            if self.lr_dev is None or opt_code < 0:
+                _lib.check(self.lib.dlrm_b200_dense_update_pack(arr, len(chunk), opt_code, lr, eps, _stream()),
+                           "dense_update_pack")
+            else:
+                _lib.check(self.lib.dlrm_b200_dense_update_pack_lr_dev(arr, len(chunk), opt_code, lr,
+                                                                       self.lr_dev.data_ptr(), eps, _stream()),
+                           "dense_update_pack_lr_dev")
             self.n_launch += 1
 
     def _tc_prepare(self, B: int):
@@ -1738,12 +1790,19 @@ class GraphedTrainSteps:
 class GraphedTrainStep:
     """One training step (forward, loss, backward, fused embedding + dense optimizer) captured
     into a CUDA graph over a static packed device batch: per step the host issues one H2D (or D2D)
-    copy of the packed inputs and one graph launch instead of ~35 kernel launches.  The learning
-    rate is baked into the graph (re-capture to change it)."""
+    copy of the packed inputs and one graph launch instead of ~35 kernel launches.  By default the
+    learning rate is baked into the graph (re-capture to change it).  device_lr=True: the optimizer
+    kernels read it from the engine's device scalar `eng.lr_scalar`, which replay(lr, lr_decay) sets
+    before every launch, so a schedule can change it from step to step.
+
+    The engine may run eager steps at other batch sizes between replays: the wgmma state the graph
+    runs on is kept (Engine._tc_keep) and restored before the next replay.  Buffers that only grow
+    (activations, occurrence lists, staging arena, scratch) must already have their final size when
+    the graph is captured: prepare the largest batch first."""
 
     def __init__(self, eng: "Engine", stage, lr: float, optimizer: str = "rwsadagrad", warmup: int = 3,
                  train: bool = True, X: Optional[torch.Tensor] = None, target: Optional[torch.Tensor] = None,
-                 pre=None):
+                 pre=None, device_lr: bool = False):
         """pre: optional callable run (and captured) before the step, e.g. the index exchange of a sharded run."""
         if train:
             _refuse_graphed_f16(eng)
@@ -1751,8 +1810,11 @@ class GraphedTrainStep:
         # table-wise sharded runs: the dense slice / targets are separate static tensors
         self.X = X if X is not None else stage.X
         self.target = target if target is not None else stage.target
-        self.lr, self.optimizer = lr, optimizer
+        self.B = self.X.shape[0]
+        self.lr, self.optimizer, self.device_lr = lr, optimizer, bool(device_lr)
         eng.ensure_optimizer_state(optimizer)
+        if self.device_lr and eng.lr_scalar is None:
+            eng.lr_scalar = torch.zeros(1, dtype=torch.float32, device=eng.device)
         if warmup > 0:
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
@@ -1763,11 +1825,20 @@ class GraphedTrainStep:
         else:
             eng.prepare(stage.sparse, train, batch=self.X.shape[0])  # allocate lazily-created buffers
         torch.cuda.synchronize()
-        n0 = eng.n_launch
+        n0, step0 = eng.n_launch, eng.opt_step
         self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self.out = self._eager()
+        if self.device_lr:
+            eng.lr_dev = eng.lr_scalar
+        try:
+            with torch.cuda.graph(self.graph):
+                self.out = self._eager()
+        finally:
+            eng.lr_dev = None
+        if self.device_lr:
+            eng.opt_step = step0        # the capture did not run a step: replay() counts them
         self.kernels_per_replay = eng.n_launch - n0
+        if eng.tc:
+            eng._tc_keep()
 
     def _eager(self):
         st = self.stage
@@ -1777,12 +1848,25 @@ class GraphedTrainStep:
             return self.eng.train_step(self.X, st.sparse, self.target, self.lr, self.optimizer)
         return self.eng.forward(self.X, st.sparse)
 
-    def replay(self):
+    def replay(self, lr: Optional[float] = None, lr_decay: float = 0.0):
+        """lr, lr_decay (device_lr graphs): the step's learning rate is computed as train_step computes it, at the
+        step this replay runs (clr = lr / (1 + (step - 1) lr_decay) for rwsadagrad and adagrad, else lr); lr=None
+        takes the lr given at capture."""
+        eng = self.eng
+        if eng.tc and eng.tc_B != self.B:
+            eng._tc_prepare(self.B)      # an eager step at another batch size ran since the last replay
+        if self.device_lr and self.train:
+            lr = self.lr if lr is None else lr
+            step = eng.opt_step + 1
+            clr = lr / (1.0 + (step - 1.0) * lr_decay) if self.optimizer in _LR_DECAY else lr
+            eng.lr_scalar.fill_(clr)
+        elif lr is not None or lr_decay:
+            raise ValueError("this graph's learning rate is baked in (capture with device_lr=True to set it per replay)")
         self.graph.replay()
-        self.eng.n_launch += self.kernels_per_replay
+        eng.n_launch += self.kernels_per_replay
         if self.train:
-            self.eng.opt_step += 1
-            self.eng._cache_dirty = bool(self.eng.cache_rows)
+            eng.opt_step += 1
+            eng._cache_dirty = bool(eng.cache_rows)
         return self.out
 
 

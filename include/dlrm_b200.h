@@ -215,6 +215,16 @@ int dlrm_b200_emb_bwd_update(const dlrm_emb_bwd_table_t* tables /*[host]*/, int 
                              const int32_t* next, const float* dY, int64_t dy_stride_sample,
                              int64_t dy_stride_table, int optimizer, float lr, float eps,
                              const dlrm_emb_dedup_t* dedup /*[host] or NULL*/, void* stream);
+/* _lr_dev variants (here and for dlrm_b200_emb_bwd_small_update, dlrm_b200_dense_update and
+ * dlrm_b200_dense_update_pack): the kernels read the learning rate from the device float *lr_dev when it is not
+ * NULL, so that a captured CUDA graph can change it between replays; lr_dev == NULL runs exactly the by-value
+ * entry point with `lr`.  The same value gives bit-identical results either way. */
+int dlrm_b200_emb_bwd_update_lr_dev(const dlrm_emb_bwd_table_t* tables /*[host]*/, int num_tables, int dim,
+                                    int64_t batch, int idx_bytes, int include_last,
+                                    const int32_t* next, const float* dY, int64_t dy_stride_sample,
+                                    int64_t dy_stride_table, int optimizer, float lr,
+                                    const float* lr_dev /*[device] or NULL*/, float eps,
+                                    const dlrm_emb_dedup_t* dedup /*[host] or NULL*/, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Table-wise sharded runs (replaces extend_distributed.alltoall, extend_distributed.py:389-486, and
@@ -358,6 +368,9 @@ int dlrm_b200_head_fused(const float* h, int64_t ldh, const float* w, const floa
 
 int dlrm_b200_dense_update(float* param, const float* grad, float* state /*NULL for SGD*/,
                            int64_t n, int optimizer, float lr, float eps, void* stream);
+int dlrm_b200_dense_update_lr_dev(float* param, const float* grad, float* state /*NULL for SGD*/,
+                                  int64_t n, int optimizer, float lr, const float* lr_dev /*[device] or NULL*/,
+                                  float eps, void* stream);
 
 
 /* ------------------------------------------------------------------------------------------
@@ -420,6 +433,8 @@ typedef struct {
 } dlrm_dense_layer_t;
 int dlrm_b200_dense_update_pack(const dlrm_dense_layer_t* layers /*[host]*/, int num_layers, int optimizer,
                                 float lr, float eps, void* stream);
+int dlrm_b200_dense_update_pack_lr_dev(const dlrm_dense_layer_t* layers /*[host]*/, int num_layers, int optimizer,
+                                       float lr, const float* lr_dev /*[device] or NULL*/, float eps, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Sharded placement (dlrm_b200/placement.py): the pieces around the gather / update kernels.
@@ -454,6 +469,12 @@ int dlrm_b200_emb_bwd_small_update(const dlrm_emb_bwd_table_t* tables /*[host]*/
                                    const float* const* peer_dY /*[host][world] or NULL*/, int world,
                                    int64_t batch_local, int64_t dy_stride_sample, int optimizer, float lr,
                                    float eps, float* scratch, int64_t scratch_bytes, void* stream);
+int dlrm_b200_emb_bwd_small_update_lr_dev(const dlrm_emb_bwd_table_t* tables /*[host]*/, int num_tables, int dim,
+                                          int64_t batch, int idx_bytes, int include_last, const float* dY,
+                                          const float* const* peer_dY /*[host][world] or NULL*/, int world,
+                                          int64_t batch_local, int64_t dy_stride_sample, int optimizer, float lr,
+                                          const float* lr_dev /*[device] or NULL*/, float eps, float* scratch,
+                                          int64_t scratch_bytes, void* stream);
 /* Row-split tables: T[b, slot_feature[s], :] = sum of the slabs [slot_first[s], slot_first[s+1]) of
  * partial ([slab][batch][dim]), in slab order. */
 int dlrm_b200_emb_reduce_partials(const float* partial, float* T, int64_t ldt, int64_t batch, int dim,
