@@ -30,7 +30,7 @@ class EmbBwdTable(C.Structure):
                 ("rows", C.c_int64), ("pair_base", C.c_int64), ("ld", C.c_int64), ("mom_stride", C.c_int64),
                 ("use_dy_off", C.c_int64), ("dy_off", C.c_int64), ("row_lo", C.c_int64), ("row_n", C.c_int64),
                 ("head_stride", C.c_int64), ("mark", C.c_void_p), ("weight_dtype", C.c_int32),
-                ("round_key", C.c_uint64)]
+                ("round_key", C.c_uint64), ("row_weights", C.c_void_p), ("row_weight_sum", C.c_void_p)]
 
 
 class EmbRemoteTable(C.Structure):

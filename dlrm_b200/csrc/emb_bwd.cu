@@ -197,9 +197,22 @@ struct EmbBwdParams {
   unsigned long long round_key[DLRM_B200_MAX_TABLES_PER_CALL];
   // learning rate in device memory (CUDA-graph steps whose rate changes between replays); NULL: lr above
   const float* lr_dev;
+  // learned weighted pooling (the RW instantiations only): v of table k and its Adagrad sum (NULL for SGD), kept out
+  // of EmbBwdTable for the same reason as round_key
+  float* row_w[DLRM_B200_MAX_TABLES_PER_CALL];
+  float* row_w_sum[DLRM_B200_MAX_TABLES_PER_CALL];
 };
 
 __device__ __forceinline__ float step_lr(const EmbBwdParams& P) { return P.lr_dev ? *P.lr_dev : P.lr; }
+
+// Learned weighted pooling: the step of the row weight v (old value v, gradient dv = <S, W_old>) and of its Adagrad
+// sum s (RWSAdagrad / Adagrad: the dense branch, as dense_update_kernel; SGD: s unused).  Returns v'.
+__device__ __forceinline__ float row_weight_step(const EmbBwdParams& P, float v, float dv, float& s) {
+  const float lr = step_lr(P);
+  if (P.optimizer == DLRM_OPT_SGD) return fmaf(-lr, dv, v);
+  s = fmaf(dv, dv, s);
+  return fmaf(-lr, dv / (sqrtf(s) + P.eps), v);
+}
 
 __device__ __forceinline__ const float* dy_row(const EmbBwdParams& P, long long bag) {
   if (P.peer_batch > 0) {
@@ -392,7 +405,9 @@ __device__ __noinline__ void dup_sum_long(const EmbBwdParams& P, int nxt, int se
 
 // EW: the element-wise Adagrad instantiation (DLRM_OPT_ADAGRAD): every lane also moves its columns of the row's
 // accumulator row, loaded with the weight row and stored with it.  EW = false is the SGD / RWSAdagrad kernel.
-template <typename wt, int W, int NV, typename idx_t, bool EW = false>
+// RW: learned weighted pooling: the owner also loads v[r] (and its sum) with the row, takes dv = <S, W_old> over the
+// warp, scales S by v[r] and steps v[r].  RW = false is the unweighted kernel unchanged.
+template <typename wt, int W, int NV, typename idx_t, bool EW = false, bool RW = false>
 __global__ void __launch_bounds__(256, NV == 1 ? (EW ? 2 : 3) : 1) emb_update_kernel(const __grid_constant__ EmbBwdParams P,
                                                                           int num_tables, long long total_hint) {
   __shared__ long long bound[DLRM_B200_MAX_TABLES_PER_CALL + 1], tend[DLRM_B200_MAX_TABLES_PER_CALL + 1];
@@ -438,6 +453,7 @@ __global__ void __launch_bounds__(256, NV == 1 ? (EW ? 2 : 3) : 1) emb_update_ke
       Pack<W> wpf[PF][NV], gpf[PF][NV];
       Pack<W> spf[EW ? PF : 1][EW ? NV : 1];     // EW: the accumulators of the lane's columns
       float mpf[PF];
+      float vpf[RW ? PF : 1], vspf[RW ? PF : 1];  // RW: v[r] and its sum (every lane loads the same word)
 #pragma unroll
       for (int u = 0; u < PF; ++u) {
         const int src = u0 + u;
@@ -462,6 +478,10 @@ __global__ void __launch_bounds__(256, NV == 1 ? (EW ? 2 : 3) : 1) emb_update_ke
             mpf[u] = 0.f;
           } else {
             mpf[u] = (P.optimizer == DLRM_OPT_RWSADAGRAD) ? tb.mom[r * tb.mom_stride] : 0.f;
+          }
+          if constexpr (RW) {
+            vpf[u] = P.row_w[ku][r];
+            vspf[u] = P.optimizer != DLRM_OPT_SGD ? P.row_w_sum[ku][r] : 0.f;
           }
         }
       }
@@ -516,6 +536,26 @@ __global__ void __launch_bounds__(256, NV == 1 ? (EW ? 2 : 3) : 1) emb_update_ke
             }
           } else {
             dup_sum_long<NV, W>(P, nxt0, self_bag, dyk_off, col_ok, g);
+          }
+        }
+        if constexpr (RW) {
+          float dv = 0.f;
+#pragma unroll
+          for (int v = 0; v < NV; ++v)
+            if (col_ok[v])
+#pragma unroll
+              for (int e = 0; e < W; ++e) dv = fmaf(g[v].x[e], w[v].x[e], dv);
+          dv = warp_sum(dv);
+          const float vr = vpf[u];
+#pragma unroll
+          for (int v = 0; v < NV; ++v)
+#pragma unroll
+            for (int e = 0; e < W; ++e) g[v].x[e] *= vr;
+          float s = vspf[u];
+          const float v_new = row_weight_step(P, vr, dv, s);
+          if (lane == 0) {
+            P.row_w[ku][r] = v_new;
+            if (P.optimizer != DLRM_OPT_SGD) P.row_w_sum[ku][r] = s;
           }
         }
         if constexpr (EW) {
@@ -645,8 +685,9 @@ __device__ __noinline__ float4 upd_sum_duplicates(const EmbBwdParams& P, int nxt
 
 // PF: row PAIRS in flight per warp.  EW: element-wise Adagrad (DLRM_OPT_ADAGRAD): every lane also loads its 8
 // accumulators (two float4 behind the row's accumulator pointer) in the same batch as the rows and stores them with
-// the row.  EW = false is the SGD / RWSAdagrad kernel.
-template <typename wt, typename idx_t, int PF, int MINB, bool EW = false>
+// the row.  EW = false is the SGD / RWSAdagrad kernel.  RW: learned weighted pooling (see emb_update_kernel): the
+// owning lanes load v[r] and its sum with the row's accumulator and store them with it.
+template <typename wt, typename idx_t, int PF, int MINB, bool EW = false, bool RW = false>
 __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid_constant__ EmbBwdParams P, int num_tables,
                                                                     long long total_hint) {
   __shared__ long long bound[DLRM_B200_MAX_TABLES_PER_CALL + 1], tend[DLRM_B200_MAX_TABLES_PER_CALL + 1];
@@ -702,6 +743,8 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
     const float* gptr = owner ? dy_row(P, bag) + tb.dy_off : nullptr;
     float* mptr = (owner && (adagrad || EW)) ? tb.mom + (long long)r * tb.mom_stride : nullptr;
     int* hptr = owner ? tb.head + (long long)r * tb.hs : nullptr;
+    float* vptr = (RW && owner) ? P.row_w[k] + r : nullptr;
+    float* vsptr = (RW && owner && P.optimizer != DLRM_OPT_SGD) ? P.row_w_sum[k] + r : nullptr;
     unsigned simple = __ballot_sync(0xffffffffu, owner && nxt == 0);
     unsigned dups = __ballot_sync(0xffffffffu, owner && nxt != 0);
 
@@ -710,6 +753,7 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
       float4 wv[PF][2], gv[PF][2];
       float4 sv[EW ? PF : 1][2];                   // EW: the lane's 8 accumulators
       float mv[PF];
+      float vv[RW ? PF : 1], vs[RW ? PF : 1];     // RW: the owning lanes' v[r] and sum
       int sa[PF], sb[PF];
 #pragma unroll
       for (int u = 0; u < PF; ++u) {
@@ -739,6 +783,10 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
         gv[u][1] = (s_ >= 0 && c1_ok && ldg) ? *reinterpret_cast<const float4*>(gp + 4) : z;
         // the owning lanes load their accumulators in the same batch as the rows
         mv[u] = (adagrad && (lane == sa[u] || lane == sb[u])) ? *mptr : 0.f;
+        if constexpr (RW) {
+          vv[u] = (lane == sa[u] || lane == sb[u]) ? *vptr : 0.f;
+          vs[u] = ((lane == sa[u] || lane == sb[u]) && vsptr) ? *vsptr : 0.f;
+        }
         if constexpr (EW) {
           const float* sp = reinterpret_cast<const float*>(__shfl_sync(0xffffffffu, (unsigned long long)mptr, sc)) + l16 * 8;
           sv[u][0] = (s_ >= 0 && c0_ok) ? *reinterpret_cast<const float4*>(sp) : z;
@@ -750,7 +798,23 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
         if (sa[u] < 0) break;
         const int s_ = half ? sb[u] : sa[u];
         const int sc = s_ < 0 ? 0 : s_;
-        const float4 g0 = gv[u][0], g1 = gv[u][1];
+        float4 g0 = gv[u][0], g1 = gv[u][1];
+        if constexpr (RW) {       // dv = <S, W_old> within the half; S *= v[r]; the owning lanes store v' and s'
+          const float4 w0 = wv[u][0], w1 = wv[u][1];
+          float dv = fmaf(g0.x, w0.x, fmaf(g0.y, w0.y, fmaf(g0.z, w0.z, g0.w * w0.w)));
+          dv = fmaf(g1.x, w1.x, fmaf(g1.y, w1.y, fmaf(g1.z, w1.z, fmaf(g1.w, w1.w, dv))));
+#pragma unroll
+          for (int o = 8; o > 0; o >>= 1) dv += __shfl_xor_sync(0xffffffffu, dv, o);
+          const float vr = __shfl_sync(0xffffffffu, vv[u], sc);
+          float s = __shfl_sync(0xffffffffu, vs[u], sc);
+          const float v_new = row_weight_step(P, vr, dv, s);
+          g0.x *= vr; g0.y *= vr; g0.z *= vr; g0.w *= vr;
+          g1.x *= vr; g1.y *= vr; g1.z *= vr; g1.w *= vr;
+          const float vA = __shfl_sync(0xffffffffu, v_new, 0), vB = __shfl_sync(0xffffffffu, v_new, 16);
+          const float sA = __shfl_sync(0xffffffffu, s, 0), sB = __shfl_sync(0xffffffffu, s, 16);
+          if (lane == sa[u]) { *vptr = vA; if (vsptr) *vsptr = sA; }
+          if (lane == sb[u]) { *vptr = vB; if (vsptr) *vsptr = sB; }
+        }
         float scale = nlr;
         if (adagrad) {
           float sq = fmaf(g0.x, g0.x, fmaf(g0.y, g0.y, fmaf(g0.z, g0.z, g0.w * g0.w)));
@@ -820,13 +884,23 @@ __global__ void __launch_bounds__(256, MINB) emb_update_lean_kernel(const __grid
       wt* wp = reinterpret_cast<wt*>(__shfl_sync(0xffffffffu, (unsigned long long)wptr, s_));
       float4 w = col_ok ? ld_row4(wp + lane * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
       const float m_old = (adagrad && lane == s_) ? *mptr : 0.f;
+      const float v_old = (RW && lane == s_) ? *vptr : 0.f;
+      const float vs_old = (RW && lane == s_ && vsptr) ? *vsptr : 0.f;
       float* spd = nullptr;
       float4 sd = make_float4(0.f, 0.f, 0.f, 0.f);
       if constexpr (EW) {
         spd = reinterpret_cast<float*>(__shfl_sync(0xffffffffu, (unsigned long long)mptr, s_)) + lane * 4;
         if (col_ok) sd = *reinterpret_cast<const float4*>(spd);
       }
-      const float4 g = upd_sum_duplicates(P, nx, (int)(base + s_), sbg, dyo, lane, col_ok);
+      float4 g = upd_sum_duplicates(P, nx, (int)(base + s_), sbg, dyo, lane, col_ok);
+      if constexpr (RW) {
+        const float dv = warp_sum(col_ok ? fmaf(g.x, w.x, fmaf(g.y, w.y, fmaf(g.z, w.z, g.w * w.w))) : 0.f);
+        const float vr = __shfl_sync(0xffffffffu, v_old, s_);
+        float s = __shfl_sync(0xffffffffu, vs_old, s_);
+        const float v_new = row_weight_step(P, vr, dv, s);
+        g.x *= vr; g.y *= vr; g.z *= vr; g.w *= vr;
+        if (lane == s_) { *vptr = v_new; if (vsptr) *vsptr = s; }
+      }
       if constexpr (EW) {
         w = adagrad_ew4(g, sd, w, nlr, P.eps);
         if (col_ok) *reinterpret_cast<float4*>(spd) = sd;
@@ -918,6 +992,8 @@ extern "C" int dlrm_b200_emb_bwd_link(const dlrm_emb_bwd_table_t* tables, int nu
 
 // Lean-kernel shape of the element-wise Adagrad instantiation: row pairs in flight per warp, CTAs per SM.
 constexpr int EW_PF = 2, EW_MINB = 2;
+// and of the learned-weight instantiation: v and its sum per row pair spill at 3 CTAs per SM (80 registers)
+constexpr int RW_PF = 2, RW_MINB = 2;
 
 static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, int dim, int64_t batch,
                            int idx_bytes, int include_last, const int32_t* next, const float* dY,
@@ -939,6 +1015,20 @@ static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, i
   if (!next || (!dY && !peer_dY)) return set_error("emb_bwd_update: NULL next/dY");
   bool vec = (dim % 4 == 0) && (peer_dY || aligned16(dY)) && dy_stride_sample % 4 == 0 && dy_stride_table % 4 == 0;
   P.flags = (dedup && dedup->flags) ? dedup->flags : nullptr;
+  bool rw = false;
+  for (int k = 0; k < num_tables; ++k) rw = rw || tables[k].row_weights != nullptr;
+  if (rw) {
+    if (peer_dY) return set_error("emb_bwd_update_p2p: row_weights (learned weighted pooling) is not supported");
+    if (P.flags) return set_error("emb_bwd_update: the duplicate filter does not support row_weights");
+    for (int k = 0; k < num_tables; ++k) {
+      if (!tables[k].row_weights)
+        return set_error("emb_bwd_update: table %d: row_weights must be set for every table of a call or for none", k);
+      if (optimizer != DLRM_OPT_SGD && !tables[k].row_weight_sum)
+        return set_error("emb_bwd_update: table %d: row_weight_sum NULL (needed by optimizer=%d)", k, optimizer);
+      P.row_w[k] = tables[k].row_weights;
+      P.row_w_sum[k] = tables[k].row_weight_sum;
+    }
+  }
   P.peer_batch = 0;
   for (int d = 0; d < DLRM_B200_MAX_PEERS; ++d) P.peer_dY[d] = nullptr;
   if (peer_dY) {
@@ -1000,14 +1090,19 @@ static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, i
   if (gridx < 1) gridx = 1;
   const long long total_hint = include_last ? 0 : (tables[num_tables - 1].pair_base + tables[num_tables - 1].nnz);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-#define UPD_E(WT, Wd, NV, EW)                                                                                \
-  do {                                                                                                           \
-    if (idx_bytes == 8)                                                                                          \
-      emb_update_kernel<WT, Wd, NV, long long, EW><<<(unsigned)gridx, block, 0, st>>>(P, num_tables, total_hint); \
-    else                                                                                                         \
-      emb_update_kernel<WT, Wd, NV, int, EW><<<(unsigned)gridx, block, 0, st>>>(P, num_tables, total_hint);      \
-    DLRM_CHECK_LAUNCH("emb_update_kernel");                                                                      \
-    return 0;                                                                                                    \
+#define UPD_R(WT, Wd, NV, EW, RW)                                                                                 \
+  do {                                                                                                               \
+    if (idx_bytes == 8)                                                                                              \
+      emb_update_kernel<WT, Wd, NV, long long, EW, RW><<<(unsigned)gridx, block, 0, st>>>(P, num_tables, total_hint); \
+    else                                                                                                             \
+      emb_update_kernel<WT, Wd, NV, int, EW, RW><<<(unsigned)gridx, block, 0, st>>>(P, num_tables, total_hint);      \
+    DLRM_CHECK_LAUNCH("emb_update_kernel");                                                                          \
+    return 0;                                                                                                        \
+  } while (0)
+#define UPD_E(WT, Wd, NV, EW)              \
+  do {                                     \
+    if (rw) UPD_R(WT, Wd, NV, EW, true);   \
+    UPD_R(WT, Wd, NV, EW, false);          \
   } while (0)
 #define UPD_T(WT, Wd, NV)   \
   do {                      \
@@ -1017,7 +1112,9 @@ static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, i
 #define UPD(Wd, NV) UPD_T(float, Wd, NV)
 #define LEAN(WT, IDX)                                                                                              \
   do {                                                                                                             \
-    if (ew) emb_update_lean_kernel<WT, IDX, EW_PF, EW_MINB, true><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint); \
+    if (ew && rw) emb_update_lean_kernel<WT, IDX, EW_PF, EW_MINB, true, true><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint); \
+    else if (ew) emb_update_lean_kernel<WT, IDX, EW_PF, EW_MINB, true><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint); \
+    else if (rw) emb_update_lean_kernel<WT, IDX, RW_PF, RW_MINB, false, true><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint); \
     else emb_update_lean_kernel<WT, IDX, 2, 3><<<(unsigned)gl, block, 0, st>>>(P, num_tables, total_hint);        \
   } while (0)
   if (f16 && !vec)
@@ -1064,6 +1161,7 @@ static int emb_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables, i
 #undef UPD
 #undef UPD_T
 #undef UPD_E
+#undef UPD_R
 }
 
 extern "C" int dlrm_b200_emb_bwd_update(const dlrm_emb_bwd_table_t* tables, int num_tables, int dim,

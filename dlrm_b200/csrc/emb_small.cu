@@ -49,6 +49,9 @@ struct SmallParams {
   int total_rows, chunks;
   unsigned long long round_key[SMALL_MAX_TABLES];   // fp16: stochastic-rounding key of table k for this step
   const float* lr_dev;  // learning rate in device memory; NULL: lr above
+  // learned weighted pooling (the RW instantiations only): v of table k and its Adagrad sum (NULL for SGD)
+  float* row_w[SMALL_MAX_TABLES];
+  float* row_w_sum[SMALL_MAX_TABLES];
 };
 
 __device__ __forceinline__ const float* small_dy_row(const SmallParams& P, long long bag) {
@@ -137,7 +140,9 @@ __global__ void __launch_bounds__(256) emb_small_accum_kernel(const __grid_const
 }
 
 // EW: element-wise Adagrad (DLRM_OPT_ADAGRAD): the lane's columns of the row's accumulator row move with the row.
-template <typename wt, int NV, bool EW = false>
+// RW: learned weighted pooling: dv = <S, W_old> over the warp, S *= v[r], then v[r] (and its sum) take their step
+// (the formulas of include/dlrm_b200.h, as emb_update_kernel).  RW = false is the unweighted kernel unchanged.
+template <typename wt, int NV, bool EW = false, bool RW = false>
 __global__ void __launch_bounds__(256) emb_small_apply_kernel(const __grid_constant__ SmallParams P, int num_tables) {
   const int lane = threadIdx.x & 31;
   const int grow = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);   // row in the partial row space
@@ -170,6 +175,32 @@ __global__ void __launch_bounds__(256) emb_small_apply_kernel(const __grid_const
   for (int v = 0; v < NV; ++v)
     if (lane * 4 + v * 128 < D) nz = nz || g[v].x != 0.f || g[v].y != 0.f || g[v].z != 0.f || g[v].w != 0.f;
   const bool touched = __any_sync(0xffffffffu, nz);
+  if constexpr (RW) {
+    // an untouched row has dv = 0 and g = 0: neither v nor its sum changes (nor the row), so nothing is rewritten
+    if (!touched) return;
+    float dv = 0.f;
+#pragma unroll
+    for (int v = 0; v < NV; ++v)
+      if (lane * 4 + v * 128 < D) {
+        const float4 w = ld_row4(wrow + v * 128);
+        dv = fmaf(g[v].x, w.x, fmaf(g[v].y, w.y, fmaf(g[v].z, w.z, fmaf(g[v].w, w.w, dv))));
+      }
+    dv = warp_sum(dv);
+    float* vp = P.row_w[k] + r;
+    const float vr = *vp;
+#pragma unroll
+    for (int v = 0; v < NV; ++v) { g[v].x *= vr; g[v].y *= vr; g[v].z *= vr; g[v].w *= vr; }
+    if (lane == 0) {
+      if (P.optimizer == DLRM_OPT_SGD) {
+        *vp = fmaf(nlr, dv, vr);
+      } else {
+        float* sp = P.row_w_sum[k] + r;
+        const float s = fmaf(dv, dv, *sp);
+        *sp = s;
+        *vp = fmaf(nlr, dv / (sqrtf(s) + P.eps), vr);
+      }
+    }
+  }
   if constexpr (EW) {
     // a row whose gradient is all zero changes neither w nor s (torch: s + 0, w + 0): not stepped, not rewritten
     if (!touched) return;
@@ -259,6 +290,12 @@ static int small_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables,
     t.ld = s.ld > 0 ? s.ld : dim; t.mom_stride = s.mom_stride > 0 ? s.mom_stride : 1;
     t.dy_off = s.dy_off; t.row_lo = s.row_n > 0 ? s.row_lo : 0; t.row_n = (int)rn; t.part_row0 = total_rows;
     P.round_key[k] = s.round_key;
+    if (!s.row_weights != !tables[0].row_weights)
+      return set_error("emb_bwd_small_update: table %d: row_weights must be set for every table of a call or for none", k);
+    if (s.row_weights && optimizer != DLRM_OPT_SGD && !s.row_weight_sum)
+      return set_error("emb_bwd_small_update: table %d: row_weight_sum NULL (needed by optimizer=%d)", k, optimizer);
+    P.row_w[k] = s.row_weights;
+    P.row_w_sum[k] = s.row_weight_sum;
     if (t.ld % 4 || (reinterpret_cast<uintptr_t>(t.w) & 15)) return set_error("emb_bwd_small_update: table %d rows not 16-byte aligned", k);
     if (ew) {     // one accumulator per element, in rows of at least dim floats on 16-byte boundaries
       t.mom_stride = s.mom_stride > 0 ? s.mom_stride : dim;
@@ -289,6 +326,14 @@ static int small_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables,
   P.partial = scratch; P.total_rows = total_rows; P.chunks = chunks;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int nv = (dim + 127) / 128;
+  const bool rw = tables[0].row_weights != nullptr;
+#define SMALL_APPLY(NV, RW)                                                                                           \
+  do {                                                                                                                \
+    if (dtype == DLRM_DTYPE_F16 && ew) emb_small_apply_kernel<__half, NV, true, RW><<<ga, 256, 0, st>>>(P, num_tables); \
+    else if (dtype == DLRM_DTYPE_F16) emb_small_apply_kernel<__half, NV, false, RW><<<ga, 256, 0, st>>>(P, num_tables); \
+    else if (ew) emb_small_apply_kernel<float, NV, true, RW><<<ga, 256, 0, st>>>(P, num_tables);                      \
+    else emb_small_apply_kernel<float, NV, false, RW><<<ga, 256, 0, st>>>(P, num_tables);                             \
+  } while (0)
 #define SMALL_LAUNCH(NV, IDX)                                                                                         \
   do {                                                                                                                \
     if (smem > 48 * 1024)                                                                                             \
@@ -297,10 +342,8 @@ static int small_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables,
     emb_small_accum_kernel<NV, IDX><<<dim3((unsigned)chunks, (unsigned)num_tables), 256, smem, st>>>(P);              \
     DLRM_CHECK_LAUNCH("emb_small_accum_kernel");                                                                      \
     const unsigned ga = (unsigned)((total_rows + 7) / 8);                                                             \
-    if (dtype == DLRM_DTYPE_F16 && ew) emb_small_apply_kernel<__half, NV, true><<<ga, 256, 0, st>>>(P, num_tables);   \
-    else if (dtype == DLRM_DTYPE_F16) emb_small_apply_kernel<__half, NV><<<ga, 256, 0, st>>>(P, num_tables);          \
-    else if (ew) emb_small_apply_kernel<float, NV, true><<<ga, 256, 0, st>>>(P, num_tables);                          \
-    else emb_small_apply_kernel<float, NV><<<ga, 256, 0, st>>>(P, num_tables);                                        \
+    if (rw) SMALL_APPLY(NV, true);                                                                                    \
+    else SMALL_APPLY(NV, false);                                                                                      \
     DLRM_CHECK_LAUNCH("emb_small_apply_kernel");                                                                      \
     return 0;                                                                                                         \
   } while (0)
@@ -313,6 +356,7 @@ static int small_update_impl(const dlrm_emb_bwd_table_t* tables, int num_tables,
   if (nv == 2) SMALL_LAUNCH(2, int);
   SMALL_LAUNCH(4, int);
 #undef SMALL_LAUNCH
+#undef SMALL_APPLY
 }
 
 extern "C" int dlrm_b200_emb_bwd_small_update(const dlrm_emb_bwd_table_t* tables, int num_tables, int dim,

@@ -102,6 +102,9 @@ class _DLRMForward(torch.autograd.Function):
         if net._fused_opt is None and eng.host:
             raise RuntimeError("dlrm_b200: host embedding tables are trained by the fused optimizers of "
                                "dlrm_b200.optim (SGD, RWSAdagrad, Adagrad); create one before calling backward()")
+        if net._fused_opt is None and net.weighted_pooling == "learned":
+            raise RuntimeError("dlrm_b200: learned weighted pooling (v_W_l) is trained by the fused optimizers of "
+                               "dlrm_b200.optim (SGD, RWSAdagrad, Adagrad); create one before calling backward()")
         if net._fused_opt is None and eng.f16:
             raise RuntimeError("dlrm_b200: fp16 embedding tables are trained by the fused optimizers of "
                                "dlrm_b200.optim (SGD, RWSAdagrad); create one before calling backward()")
@@ -157,8 +160,6 @@ class DLRM_Net(nn.Module):
         self.loss_function = loss_function
         self.weighted_pooling = ("learned" if weighted_pooling is not None and weighted_pooling != "fixed"
                                  else weighted_pooling)
-        if self.weighted_pooling == "learned":
-            sys.exit("ERROR: learned weighted pooling is not supported by dlrm_b200 (fixed only)")
         self.qr_flag, self.md_flag = False, False
         self.quantize_emb, self.emb_l_q, self.quantize_bits = False, [], 32
         ln_emb = np.asarray(ln_emb).astype(np.int64)
@@ -224,7 +225,8 @@ class DLRM_Net(nn.Module):
                                   max_batch=max_batch, gemm=gemm, emb_dtype=emb_dtype, round_seed=round_seed,
                                   interleave_momentum=None if emb_dtype == "fp16" else False, host_tables=host,
                                   host_cache_rows=emb_host_cache or 0,
-                                  host_cache_reserve=self.host_reserve(m_spa, ln_emb))
+                                  host_cache_reserve=self.host_reserve(m_spa, ln_emb),
+                                  learned_row_weights=self.weighted_pooling == "learned")
         self._m_spa, self._ln_emb = int(m_spa), ln_emb
         # same construction (and numpy RNG consumption) order as the reference: tables, bottom, top
         if ndevices <= 1:
@@ -338,9 +340,15 @@ class DLRM_Net(nn.Module):
             emb_l.append(_TableView(tab))
             if weighted_pooling is None:
                 v_W_l.append(None)
-            else:
+            elif not eng.learned_row_weights:
                 v_W_l.append(torch.ones(n, dtype=torch.float32, device=eng.device))
-        if weighted_pooling is not None:
+        if weighted_pooling is not None and eng.learned_row_weights:
+            # Parameters that share storage with the engine's arena (ones, as the reference's torch.ones(n)): the fused
+            # update steps them, state_dict() reads and load_state_dict() writes the arena
+            eng.row_weights.fill_(1.0)
+            v_W_l = nn.ParameterList([nn.Parameter(eng.row_weights[int(eng.row_base[k]):int(eng.row_base[k + 1])])
+                                      for k in range(ln.size)])
+        elif weighted_pooling is not None:
             eng.row_weights = torch.cat(v_W_l)
             v_W_l = [eng.row_weights[int(eng.row_base[k]):int(eng.row_base[k + 1])] for k in range(ln.size)]
         return emb_l, v_W_l

@@ -102,7 +102,7 @@ class Engine:
                  max_batch: int = 2048, gemm: str = "simt", n_features: Optional[int] = None,
                  interleave_momentum: Optional[bool] = None, shards=None, split_slots=None, small_rows_max: int = 256,
                  emb_dtype: str = "fp32", round_seed: int = 0, host_tables: Sequence[int] = (),
-                 host_cache_rows=0, host_cache_reserve: int = 1 << 31):
+                 host_cache_rows=0, host_cache_reserve: int = 1 << 31, learned_row_weights: bool = False):
         if not torch.cuda.is_available():
             raise RuntimeError("dlrm_b200.Engine needs a CUDA device (H100, sm_90a); there is no CPU path")
         self.device = torch.device(device)
@@ -212,6 +212,13 @@ class Engine:
         self._momentum_sep: Optional[torch.Tensor] = None
         self.acc_ew: Optional[torch.Tensor] = None       # element-wise Adagrad accumulators [total_rows, D]
         self.row_weights: Optional[torch.Tensor] = None  # weighted pooling v_W_l, arena [total_rows]
+        # Learned weighted pooling (--weighted-pooling=learned): v starts at one and the fused update steps it with its
+        # rows (dv = <S, W_old>); RWSAdagrad / Adagrad keep its dense 'sum' in row_weight_sum [total_rows].
+        self.learned_row_weights = bool(learned_row_weights)
+        self.row_weight_sum: Optional[torch.Tensor] = None
+        if self.learned_row_weights:
+            self._check_learned_placement()
+            self.row_weights = torch.ones(self.total_rows, dtype=torch.float32, device=dev)
         # ---- dense arena
         self.dense_slices = []  # (name, layer, kind, offset, shape)
         ofs = 0
@@ -707,6 +714,13 @@ class Engine:
         """Row-wise Adagrad accumulator of every row, [sum rows] fp32 (a strided view when interleaved)."""
         return self.tables.view(torch.float32)[:, self._meta_col] if self.interleave else self._momentum_sep
 
+    def _check_learned_placement(self):
+        """Learned row weights are indexed by the table row: every table whole and in device memory."""
+        if self.host:
+            raise ValueError("host tables do not support weighted pooling: row_weights is indexed by the table row")
+        if any(int(s["nparts"]) > 1 or int(s["table"]) != k for k, s in enumerate(self.shards)):
+            raise ValueError("learned weighted pooling is not supported on sharded runs")
+
     def ensure_optimizer_state(self, optimizer: str):
         if optimizer == "rwsadagrad":
             if not self.interleave and self._momentum_sep is None:
@@ -722,6 +736,12 @@ class Engine:
                 self.acc_ew_h = self._pinned_zeros((self.host_rows, self.D))
         if optimizer in _LR_DECAY and self.dense_state is None:
             self.dense_state = torch.zeros_like(self.dense)
+        if optimizer in _LR_DECAY and self.learned_row_weights and self.row_weight_sum is None:
+            self.row_weight_sum = torch.zeros(self.total_rows, dtype=torch.float32, device=self.device)
+
+    def row_weight_sum_of(self, k: int) -> torch.Tensor:
+        """[rows_k] Adagrad 'sum' of the learned row weights of table k (after ensure_optimizer_state)."""
+        return self.row_weight_sum[int(self.row_base[k]):int(self.row_base[k + 1])]
 
     def accumulator_ew(self, k: int) -> torch.Tensor:
         """[rows_k, D] element-wise Adagrad accumulators of table k (after ensure_optimizer_state("adagrad"))."""
@@ -757,7 +777,8 @@ class Engine:
                     self.W[name][i].copy_(torch.as_tensor(Wl, dtype=torch.float32))
                     self.b[name][i].copy_(torch.as_tensor(bl, dtype=torch.float32))
             if params.get("v_W_l") is not None:
-                self.row_weights = torch.empty(self.total_rows, dtype=torch.float32, device=self.device)
+                if self.row_weights is None:    # learned weights: written in place (parameters are views)
+                    self.row_weights = torch.empty(self.total_rows, dtype=torch.float32, device=self.device)
                 for k, w in enumerate(params["v_W_l"]):
                     self.row_weights[int(self.row_base[k]):int(self.row_base[k + 1])].copy_(
                         torch.as_tensor(w, dtype=torch.float32))
@@ -869,6 +890,10 @@ class Engine:
                 d.indices, d.rows = self._slot_ptr(sp, k), self._arena_rows
             d.pair_base = 0 if sp.include_last else base
             base += sp.indices[k].numel()
+            if self.learned_row_weights:
+                d.row_weights = self.row_weights.data_ptr() + int(self.row_base[k]) * 4
+                d.row_weight_sum = (self.row_weight_sum.data_ptr() + int(self.row_base[k]) * 4
+                                    if self.row_weight_sum is not None else None)
         total = sp.nnz_total if sp.include_last else base
         return arr, total
 

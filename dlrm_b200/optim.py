@@ -12,6 +12,7 @@ on the device.  `param_groups[0]["lr"]` is honoured every step, so `LRPolicySche
 """
 from __future__ import annotations
 
+import numpy as np
 import torch
 
 
@@ -66,14 +67,20 @@ class _Fused(torch.optim.Optimizer):
 
     # ------------------------------------------------------------------ checkpoint (opt_state_dict)
     def _state_view(self, p):
-        """('momentum', [rows] view) for an embedding table, ('sum', same-shape view) for an MLP parameter: the
-        engine memory that holds the reference's per-parameter state (optim/rwsadagrad.py:86-100).  Adagrad:
-        ('sum', [rows, D] view) for an embedding table too (torch.optim.Adagrad's state)."""
+        """('momentum', [rows] view) for an embedding table, ('sum', same-shape view) for an MLP parameter or a
+        learned row-weight vector v_W_l[k]: the engine memory that holds the reference's per-parameter state
+        (optim/rwsadagrad.py:86-100).  Adagrad: ('sum', [rows, D] view) for an embedding table too
+        (torch.optim.Adagrad's state)."""
         eng = self.net._engine
         lo = eng.dense.data_ptr()
         if lo <= p.data_ptr() < lo + eng.dense.numel() * 4:
             off = (p.data_ptr() - lo) // 4
             return "sum", eng.dense_state[off:off + p.numel()].view(p.shape)
+        if getattr(self.net, "weighted_pooling", None) == "learned":
+            lo = eng.row_weights.data_ptr()
+            if lo <= p.data_ptr() < lo + eng.row_weights.numel() * 4:
+                k = int(np.searchsorted(eng.row_base, (p.data_ptr() - lo) // 4, side="right")) - 1
+                return "sum", eng.row_weight_sum_of(k)
         for k in range(len(eng.row_base) - 1):
             if eng.table(k).data_ptr() == p.data_ptr():
                 if self._name == "adagrad":

@@ -132,6 +132,17 @@ int dlrm_b200_emb_bag_fwd(const dlrm_emb_fwd_table_t* tables /*[host]*/, int num
  * |x| > 65504 -> +-inf, NaN stays NaN.  r = 16 bits of h = splitmix64(round_key ^ R * 0xC2B2AE3D27D4EB4F ^
  * (c / 4) * 0x165667B19E3779F9) for global row R = row_lo + local row and column c: bits [16 (c % 4), +16) of h.
  * Rows that are not updated are not rewritten.
+ * Learned weighted pooling (row_weights != NULL, v = v_W_l[k] of dlrm_s_pytorch.py:425-428): the forward pooled
+ * v[row] * W[row] per occurrence, so with S = the coalesced sum of dY above (v scales every occurrence alike)
+ *               g      = v[row] * S                              (fp32 product per element; the step above takes g)
+ *               dv     = <S, W_old[row]>                         (the row BEFORE its step; fp16: the widened row)
+ *   SGD:        v[row] = fmaf(-lr, dv, v[row])
+ *   RWSAdagrad, Adagrad (the dense branch of optim/rwsadagrad.py:145-148 and torch.optim.Adagrad on the [rows]
+ *   parameter v; both keep a [rows] 'sum'):
+ *               s = fmaf(dv, dv, row_weight_sum[row]);  v[row] = fmaf(-lr, dv / (sqrtf(s) + eps), v[row])
+ * with the same lr as the rows.  Only the owner of a row writes v[row] and row_weight_sum[row]: the entries of rows
+ * that do not occur stay bit-identical (their gradient is 0 in the reference).  row_weights == NULL runs the
+ * unweighted kernels unchanged.  The duplicate filter and dlrm_b200_emb_bwd_update_p2p refuse row_weights.
  * dY[b, k, :] is read at dY + b*dy_stride_sample + k*dy_stride_table.
  * ------------------------------------------------------------------------------------------ */
 typedef struct {
@@ -173,6 +184,11 @@ typedef struct {
   /* fp16 only: stochastic-rounding key of this table for this step (see above), the hash prefix
    * splitmix64(seed * 0xD6E8FEB86659FD93 ^ (step + 1) * 0x9E3779B97F4A7C15 ^ (global table + 1) * 0x165667B19E3779F9) */
   uint64_t round_key;
+  /* learned weighted pooling (see above): [rows] fp32 v of this table (local rows of a shard), read and updated in
+   * place, or NULL (unweighted, or fixed weights of one); row_weight_sum: [rows] fp32 Adagrad 'sum' of v for
+   * RWSAdagrad / Adagrad, NULL for SGD.  Ignored by the training gather. */
+  float* row_weights;
+  float* row_weight_sum;
 } dlrm_emb_bwd_table_t;
 
 /* Optional duplicate filter (dlrm_emb_dedup_t): at 1e6-row tables almost every row of a batch is
