@@ -13,7 +13,7 @@ ACT_NONE, ACT_RELU, ACT_SIGMOID = 0, 1, 2
 LOSS_MSE, LOSS_BCE, LOSS_WBCE = 0, 1, 2
 OPT_SGD, OPT_RWSADAGRAD, OPT_ADAGRAD = 0, 1, 2
 GEMM_SIMT_FP32, GEMM_TC_BF16X3, GEMM_TC_BF16 = 0, 1, 2
-DTYPE_F32, DTYPE_F16 = 0, 1
+DTYPE_F32, DTYPE_F16, DTYPE_Q8, DTYPE_Q4 = 0, 1, 2, 3
 TUNE = dict(emb_bags_per_group=0, emb_unroll=1, head_rows=6, interact_bwd_cols=7, pdl=8, upd_lean=10, upd_debug=11)
 
 
@@ -102,7 +102,7 @@ SYMBOLS = [
     "dlrm_b200_host_stage_in", "dlrm_b200_host_write_back", "dlrm_b200_host_release", "dlrm_b200_host_register",
     "dlrm_b200_host_unregister", "dlrm_b200_host_cache_flush",
     "dlrm_b200_emb_bwd_update_lr_dev", "dlrm_b200_emb_bwd_small_update_lr_dev", "dlrm_b200_dense_update_lr_dev",
-    "dlrm_b200_dense_update_pack_lr_dev",
+    "dlrm_b200_dense_update_pack_lr_dev", "dlrm_b200_emb_quantize_rows",
 ]
 
 
@@ -175,6 +175,7 @@ def _declare(lib):
                                                           C.POINTER(vp), i32, i64, i64, i32, f32, vp, f32, vp, i64, vp]
     lib.dlrm_b200_dense_update_lr_dev.argtypes = [vp, vp, vp, i64, i32, f32, vp, f32, vp]
     lib.dlrm_b200_dense_update_pack_lr_dev.argtypes = [C.POINTER(DenseLayer), i32, i32, f32, vp, f32, vp]
+    lib.dlrm_b200_emb_quantize_rows.argtypes = [vp, i32, i64, i64, i32, vp, i32, i64, vp]
     for name in SYMBOLS:
         fn = getattr(lib, name)
         if name in ("dlrm_b200_head_scratch_bytes", "dlrm_b200_emb_bwd_small_scratch_bytes"):

@@ -237,8 +237,21 @@ def run(argv=None):
         if args.data_generation in ("random", "synthetic"):
             sys.exit("ERROR: --cuda-graph-steps needs --data-generation=dataset (the random generator de-duplicates "
                      "each bag, so the number of indices changes from batch to batch)")
-    if args.quantize_emb_with_bit in [4, 8] or args.quantize_mlp_with_bit != 32:
+    # --inference-only --quantize-emb-with-bit=4|8 (dlrm_s_pytorch.py:1458-1483): the tables are built as packed row-wise
+    # quantized rows (DLRM_Net(emb_dtype="int8" | "int4")) and a --load-model checkpoint is quantized as it loads.  The
+    # reference ignores the flag when it trains and has no quantized MLPs on the GPU.
+    quant_emb = args.quantize_emb_with_bit in [4, 8]
+    if (quant_emb and not args.inference_only) or args.quantize_mlp_with_bit != 32:
         sys.exit("ERROR: 4 and 8-bit quantization on GPU is not supported")
+    if quant_emb:
+        if args.emb_dtype == "fp16":
+            sys.exit("ERROR: --quantize-emb-with-bit replaces the table storage type: it does not combine with "
+                     "--emb-dtype=fp16 (fp16 checkpoints still load)")
+        if args.emb_host_tables:
+            sys.exit("ERROR: --quantize-emb-with-bit keeps the packed tables in device memory (--emb-host-tables is "
+                     "not supported)")
+        if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+            sys.exit("ERROR: --quantize-emb-with-bit runs on one GPU (sharded runs are not supported)")
     if not torch.cuda.is_available():
         sys.exit("ERROR: dlrm_b200 needs a CUDA device (there is no CPU path); the reference covers CPU runs")
     np.random.seed(args.numpy_rand_seed)
@@ -440,7 +453,8 @@ def run(argv=None):
                     loss_threshold=args.loss_threshold, ndevices=-1, weighted_pooling=args.weighted_pooling,
                     loss_function=args.loss_function, device=device, gemm=args.gemm,
                     max_batch=args.mini_batch_size, loss_weights=loss_ws,
-                    emb_dtype=torch.float16 if args.emb_dtype == "fp16" else torch.float32,
+                    emb_dtype=(("int8" if args.quantize_emb_with_bit == 8 else "int4") if quant_emb
+                               else torch.float16 if args.emb_dtype == "fp16" else torch.float32),
                     emb_host_tables=host_tables or None, emb_host_cache=host_cache or None)
     optimizer = lr_scheduler = None
     if not args.inference_only:
@@ -480,8 +494,9 @@ def run(argv=None):
     total_time = total_loss = total_iter = total_samp = 0
     if args.load_model:                                      # dlrm_s_pytorch.py:1399-1456
         print("Loading saved model {}".format(args.load_model))
-        # host tables: the checkpoint's tables stay in (memory-mapped) host memory; load_state_dict copies them in place
-        ld = (torch.load(args.load_model, map_location="cpu", mmap=True, weights_only=False) if host_tables
+        # host tables: the checkpoint's tables stay in (memory-mapped) host memory; load_state_dict copies them in place.
+        # Quantized tables: the float tables stay there too and cross to the device one chunk at a time.
+        ld = (torch.load(args.load_model, map_location="cpu", mmap=True, weights_only=False) if host_tables or quant_emb
               else torch.load(args.load_model, map_location=device, weights_only=False))
         dlrm.load_state_dict(ld["state_dict"])
         ld_j, ld_k = ld["iter"], ld["epoch"]
@@ -514,6 +529,10 @@ def run(argv=None):
         test_B = args.test_mini_batch_size if (args.inference_only or args.test_freq > 0) else None
         graphs = GraphSteps(dlrm, optimizer, args.mini_batch_size, test_B, m_den, args.optimizer)
     score_keys = None
+
+    def sd():
+        # a quantized model has no float tables to save; its runs are inference-only and write no checkpoint
+        return None if quant_emb else dlrm.state_dict()
 
     def inference(best_acc, best_auc=0.0):
         """One pass over the test set (inference(), dlrm_s_pytorch.py:759-900): accuracy of round(Z) against the
@@ -554,7 +573,7 @@ def run(argv=None):
         if args.mlperf_logging:
             res = score_keys.finalize()
             metrics = {"nepochs": args.nepochs, "nbatches": nbatches, "nbatches_test": nbatches_test,
-                       "state_dict": dlrm.state_dict(), "test_acc": res["accuracy"]}
+                       "state_dict": sd(), "test_acc": res["accuracy"]}
             is_best = res["roc_auc"] > best_auc
             if is_best:
                 best_auc = res["roc_auc"]
@@ -567,7 +586,7 @@ def run(argv=None):
             return metrics, is_best, res
         acc = test_accu / test_samp
         metrics = {"nepochs": args.nepochs, "nbatches": nbatches, "nbatches_test": nbatches_test,
-                   "state_dict": dlrm.state_dict(), "test_acc": acc}
+                   "state_dict": sd(), "test_acc": acc}
         is_best = acc > best_acc
         if is_best:
             best_acc = acc

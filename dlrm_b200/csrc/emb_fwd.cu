@@ -11,9 +11,57 @@
 // (c) 8..16 warps per CTA x many CTAs per SM.
 // fp16 tables (template row type wt = __half): the same lanes load 4 halves (8 bytes) instead of a float4 and
 // widen them, so every column is still summed in fp32 in index order (== the fp32 gather over the widened table).
+// Row-wise quantized tables (wt = q8_t / q4_t, forward only): the same lanes load 4 levels (4 bytes / 2 bytes) and
+// the row's scale and bias, and add acc = fma(s, q, acc + b) column by column in index order -- the sum of
+// torch.ops.quantized.embedding_bag_{byte,4bit}_rowwise_offsets on the CPU, bit for bit.
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace dlrm {
+
+// Packed row types of DLRM_DTYPE_Q8 / Q4 (include/dlrm_b200.h): one byte per element, so W + r * ld is row r.
+struct q8_t { unsigned char b; };
+struct q4_t { unsigned char b; };
+template <typename wt>
+struct is_quant { static constexpr bool value = std::is_same<wt, q8_t>::value || std::is_same<wt, q4_t>::value; };
+
+// the packed levels of columns [c, c + 4) of a row (c % 4 == 0): 4 bytes (8-bit) or 2 bytes (4-bit), kept packed in
+// one register until they are added (a float4 per row in flight would spill the 64-register dim-128 kernel)
+template <typename wt>
+__device__ __forceinline__ unsigned ldg_qlevels4(const unsigned char* row, int c) {
+  if constexpr (std::is_same<wt, q8_t>::value) return __ldg(reinterpret_cast<const unsigned*>(row + c));
+  else return __ldg(reinterpret_cast<const unsigned short*>(row + c / 2));
+}
+template <typename wt>
+__device__ __forceinline__ float4 qlevels_f4(unsigned u) {
+  if constexpr (std::is_same<wt, q8_t>::value)
+    return make_float4((float)(u & 255u), (float)((u >> 8) & 255u), (float)((u >> 16) & 255u), (float)(u >> 24));
+  else   // column 2j in the low nibble of byte j
+    return make_float4((float)(u & 15u), (float)((u >> 4) & 15u), (float)((u >> 8) & 15u), (float)((u >> 12) & 15u));
+}
+// one level of a packed row
+template <typename wt>
+__device__ __forceinline__ float ldg_qlevel(const unsigned char* row, int c) {
+  if constexpr (std::is_same<wt, q8_t>::value) return (float)__ldg(row + c);
+  else return (float)((__ldg(row + c / 2) >> (4 * (c & 1))) & 15);
+}
+// (scale, bias) of a packed row of D columns, widened to fp32
+template <typename wt>
+__device__ __forceinline__ float2 ldg_qscale_bias(const unsigned char* row, int D) {
+  if constexpr (std::is_same<wt, q8_t>::value) {
+    const float* sb = reinterpret_cast<const float*>(row + D);
+    return make_float2(__ldg(sb), __ldg(sb + 1));
+  } else {
+    return __half22float2(__ldg(reinterpret_cast<const __half2*>(row + D / 2)));
+  }
+}
+// acc + w * (scale * q + bias) the way the CPU op adds it: s = scale * w and b = bias * w rounded first, then
+// fma(s, q, acc + b); nothing is contracted
+__device__ __forceinline__ float4 qaccum4(float4 acc, float4 q, float s, float b) {
+  return make_float4(__fmaf_rn(s, q.x, __fadd_rn(acc.x, b)), __fmaf_rn(s, q.y, __fadd_rn(acc.y, b)),
+                     __fmaf_rn(s, q.z, __fadd_rn(acc.z, b)), __fmaf_rn(s, q.w, __fadd_rn(acc.w, b)));
+}
 
 struct EmbFwdTable {
   const void* w;        // rows of the table's row type (float or __half)
@@ -158,14 +206,24 @@ __global__ void __launch_bounds__(256, (G == 32 && NV == 1) ? 4 : 1) emb_fwd_vec
         for (int jj = 0; jj < n; jj += U) {
           float4 val[U][NV];
           float wgt[U];
+          unsigned qv[U][NV];   // quantized rows: packed levels
+          float2 qsb[U];        //                 (scale, bias)
 #pragma unroll
           for (int u = 0; u < U; ++u) {
             const long long r = __shfl_sync(gmask, my_row, jj + u, G);  // jj+u < G always (U | G)
             if (jj + u < n) {
-              const wt* rp = W + r * tb.ld + gl * 4;
+              if constexpr (is_quant<wt>::value) {
+                const unsigned char* rb = reinterpret_cast<const unsigned char*>(W + r * tb.ld);
 #pragma unroll
-              for (int v = 0; v < NV; ++v) {
-                if (gl * 4 + v * G * 4 < D) val[u][v] = ldg_stream_row4(rp + v * G * 4);
+                for (int v = 0; v < NV; ++v)
+                  if (gl * 4 + v * G * 4 < D) qv[u][v] = ldg_qlevels4<wt>(rb, gl * 4 + v * G * 4);
+                qsb[u] = ldg_qscale_bias<wt>(rb, D);
+              } else {
+                const wt* rp = W + r * tb.ld + gl * 4;
+#pragma unroll
+                for (int v = 0; v < NV; ++v) {
+                  if (gl * 4 + v * G * 4 < D) val[u][v] = ldg_stream_row4(rp + v * G * 4);
+                }
               }
               if (WEIGHTED) wgt[u] = __ldg(tb.rw + r);
             }
@@ -173,6 +231,13 @@ __global__ void __launch_bounds__(256, (G == 32 && NV == 1) ? 4 : 1) emb_fwd_vec
 #pragma unroll
           for (int u = 0; u < U; ++u) {
             if (jj + u < n) {
+              if constexpr (is_quant<wt>::value) {
+                const float s = WEIGHTED ? __fmul_rn(qsb[u].x, wgt[u]) : qsb[u].x;
+                const float b = WEIGHTED ? __fmul_rn(qsb[u].y, wgt[u]) : qsb[u].y;
+#pragma unroll
+                for (int v = 0; v < NV; ++v) acc[v] = qaccum4(acc[v], qlevels_f4<wt>(qv[u][v]), s, b);
+                continue;
+              }
 #pragma unroll
               for (int v = 0; v < NV; ++v) {
                 if (WEIGHTED) {
@@ -397,8 +462,16 @@ __global__ void emb_fwd_scalar_kernel(const __grid_constant__ EmbFwdParams P) {
       if (prev) tb.mark[prev - 1] = 1;
     }
     if (!mine) continue;
-    const float x = (float)static_cast<const wt*>(tb.w)[r * tb.ld + d];
-    acc = WEIGHTED ? fmaf(tb.rw[r], x, acc) : acc + x;
+    if constexpr (is_quant<wt>::value) {
+      const unsigned char* rb = reinterpret_cast<const unsigned char*>(static_cast<const wt*>(tb.w) + r * tb.ld);
+      const float2 sb = ldg_qscale_bias<wt>(rb, D);
+      const float s = WEIGHTED ? __fmul_rn(sb.x, tb.rw[r]) : sb.x;
+      const float b = WEIGHTED ? __fmul_rn(sb.y, tb.rw[r]) : sb.y;
+      acc = __fmaf_rn(s, ldg_qlevel<wt>(rb, d), __fadd_rn(acc, b));
+    } else {
+      const float x = (float)static_cast<const wt*>(tb.w)[r * tb.ld + d];
+      acc = WEIGHTED ? fmaf(tb.rw[r], x, acc) : acc + x;
+    }
   }
   out_ptr(P, tb, b)[d] = acc;
 }
@@ -409,10 +482,12 @@ static int launch_vec(const EmbFwdParams& P, int num_tables, bool shard, cudaStr
   const long long groups_per_block = (long long)(block / 32) * (32 / G);
   const long long groups = (P.batch + P.bags_per_group - 1) / P.bags_per_group;
   dim3 grid((unsigned)((groups + groups_per_block - 1) / groups_per_block), (unsigned)num_tables);
-  if (shard) {
-    emb_fwd_shard_kernel<wt, G, NV, U, idx_t, WEIGHTED, LINK><<<grid, block, 0, st>>>(P, num_tables);
-    DLRM_CHECK_LAUNCH("emb_fwd_shard_kernel");
-    return 0;
+  if constexpr (!is_quant<wt>::value) {   // quantized tables are whole tables (refused before dispatch)
+    if (shard) {
+      emb_fwd_shard_kernel<wt, G, NV, U, idx_t, WEIGHTED, LINK><<<grid, block, 0, st>>>(P, num_tables);
+      DLRM_CHECK_LAUNCH("emb_fwd_shard_kernel");
+      return 0;
+    }
   }
   emb_fwd_vec_kernel<wt, G, NV, U, idx_t, WEIGHTED, LINK><<<grid, block, 0, st>>>(P, num_tables);
   DLRM_CHECK_LAUNCH("emb_fwd_vec_kernel");
@@ -469,8 +544,14 @@ static int emb_fwd_impl(const dlrm_emb_fwd_table_t* tables, const dlrm_emb_bwd_t
   EmbFwdParams P;
   bool weighted = false, any_unweighted = false, any_shard = false;
   const int dtype = num_tables > 0 ? tables[0].weight_dtype : DLRM_DTYPE_F32;
-  if (dtype != DLRM_DTYPE_F32 && dtype != DLRM_DTYPE_F16) return set_error("emb_bag_fwd: weight_dtype=%d", dtype);
+  const bool quant = dtype == DLRM_DTYPE_Q8 || dtype == DLRM_DTYPE_Q4;
+  if (dtype != DLRM_DTYPE_F32 && dtype != DLRM_DTYPE_F16 && !quant) return set_error("emb_bag_fwd: weight_dtype=%d", dtype);
   if (dtype == DLRM_DTYPE_F16 && dim % 8) return set_error("emb_bag_fwd: fp16 tables need dim %% 8 == 0 (dim=%d)", dim);
+  if ((dtype == DLRM_DTYPE_Q8 && dim % 4) || (dtype == DLRM_DTYPE_Q4 && dim % 8))
+    return set_error("emb_bag_fwd: quantized tables need dim %% %d == 0 (dim=%d)", dtype == DLRM_DTYPE_Q8 ? 4 : 8, dim);
+  if (quant && (train || peer_out))
+    return set_error("emb_bag_fwd: quantized tables are forward-only and local (no training gather, no peer stores)");
+  const long long qwidth = dtype == DLRM_DTYPE_Q8 ? dim + 8 : dim / 2 + 4;   // packed row bytes
   bool vec_ok = (dim % 4 == 0) && dim <= 512 && (peer_out || aligned16(out)) && out_stride_sample % 4 == 0 &&
                 out_stride_table % 4 == 0;
   for (int k = 0; k < num_tables; ++k) {
@@ -481,8 +562,10 @@ static int emb_fwd_impl(const dlrm_emb_fwd_table_t* tables, const dlrm_emb_bwd_t
     P.t[k].off = tables[k].offsets;
     P.t[k].rw = tables[k].row_weights;
     P.t[k].nnz = tables[k].nnz;
-    P.t[k].ld = tables[k].ld > 0 ? tables[k].ld : dim;
-    if (P.t[k].ld < dim) return set_error("emb_bag_fwd: table %d: ld=%lld < dim", k, (long long)tables[k].ld);
+    P.t[k].ld = tables[k].ld > 0 ? tables[k].ld : (quant ? qwidth : dim);
+    if (P.t[k].ld < (quant ? qwidth : dim)) return set_error("emb_bag_fwd: table %d: ld=%lld < row width", k, (long long)tables[k].ld);
+    if (quant && (P.t[k].ld % 4 || (reinterpret_cast<uintptr_t>(tables[k].weight) & 3)))
+      return set_error("emb_bag_fwd: table %d: quantized rows need a 4-byte aligned base and ld %% 4 == 0", k);
     vec_ok = vec_ok && (P.t[k].ld % 4 == 0);
     P.t[k].head = train ? train[k].head : nullptr;   // train[k].head == NULL: this table is not linked
     P.t[k].hs = (train && train[k].head_stride > 0) ? train[k].head_stride : 1;
@@ -501,13 +584,14 @@ static int emb_fwd_impl(const dlrm_emb_fwd_table_t* tables, const dlrm_emb_bwd_t
       return set_error("emb_bag_fwd: table %d: row range [%lld, +%lld) outside %lld rows", k,
                        (long long)P.t[k].row_lo, (long long)P.t[k].row_n, (long long)tables[k].rows);
     any_shard = any_shard || P.t[k].row_lo != 0 || P.t[k].row_n != P.t[k].rows;
+    if (quant && any_shard) return set_error("emb_bag_fwd: table %d: quantized tables are whole tables (no row range)", k);
     if (!tables[k].weight || !tables[k].offsets || (!tables[k].indices && tables[k].nnz > 0))
       return set_error("emb_bag_fwd: table %d has a NULL pointer", k);
     if (tables[k].nnz > 0x7ffffffeLL) return set_error("emb_bag_fwd: table %d: nnz >= 2^31 per call", k);
     if (train && train[k].pair_base + tables[k].nnz > 0x7ffffffeLL)
       return set_error("emb_bag_fwd_train: more than 2^31-2 index occurrences");
     if (tables[k].row_weights) weighted = true; else any_unweighted = true;
-    vec_ok = vec_ok && aligned16(tables[k].weight);
+    vec_ok = vec_ok && (quant || aligned16(tables[k].weight));
   }
   if (weighted && any_unweighted)
     return set_error("emb_bag_fwd: row_weights must be given for all tables of a call or none");
@@ -554,6 +638,18 @@ static int emb_fwd_impl(const dlrm_emb_fwd_table_t* tables, const dlrm_emb_bwd_t
     if (idx_bytes == 8) DISPATCH(__half, long long);
     DISPATCH(__half, int);
   }
+#define DISPATCH_Q(WT, IDX)                                                                      \
+  return weighted ? dispatch<WT, IDX, true, false>(P, num_tables, vec_ok, false, st)             \
+                  : dispatch<WT, IDX, false, false>(P, num_tables, vec_ok, false, st)
+  if (dtype == DLRM_DTYPE_Q8) {
+    if (idx_bytes == 8) DISPATCH_Q(q8_t, long long);
+    DISPATCH_Q(q8_t, int);
+  }
+  if (dtype == DLRM_DTYPE_Q4) {
+    if (idx_bytes == 8) DISPATCH_Q(q4_t, long long);
+    DISPATCH_Q(q4_t, int);
+  }
+#undef DISPATCH_Q
   if (idx_bytes == 8) DISPATCH(float, long long);
   DISPATCH(float, int);
 #undef DISPATCH

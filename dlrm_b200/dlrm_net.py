@@ -26,8 +26,12 @@ memory.  `emb_host_cache=N | "auto"` also keeps up to N of their rows in HBM bet
 cache, least recently used way replaced; "auto": the device memory free at the first batch beyond `host_reserve`).
 A cached row's host copy is then stale: `emb_l[k].weight` of a host table shows the current rows only after
 `state_dict()`, `load_state_dict()`, `engine.table(k)` or the optimizer's `state_dict()`, which write the cache back
-(and empty it).  A training loop that calls none of them never writes it back.  QR / mixed-dimension embeddings, quantised embeddings and `parallel_forward` are outside the path
+(and empty it).  A training loop that calls none of them never writes it back.  QR / mixed-dimension embeddings and `parallel_forward` are outside the path
 (SURVEY §2) and exit with an error when requested.
+Row-wise quantized tables (inference only): `quantize_embedding(bits)` packs the float tables into fbgemm's 8- or 4-bit
+rows, `emb_l_q[k]`, and the forward pools those from then on (the float tables stay).  `emb_dtype="int8" | "int4"` builds
+a model whose float tables are never allocated: the initial draw and `load_state_dict` quantize each table as it is
+written, and `state_dict()` is refused.  Either way the pooled rows are bit-identical to the reference's CPU ops.
 """
 from __future__ import annotations
 
@@ -141,10 +145,16 @@ class DLRM_Net(nn.Module):
             emb_dtype = "fp16"
         elif emb_dtype in (torch.float32, "fp32", "float32"):
             emb_dtype = "fp32"
-        else:
-            sys.exit("ERROR: emb_dtype must be torch.float32 or torch.float16")
+        elif emb_dtype not in ("int8", "int4"):
+            sys.exit("ERROR: emb_dtype must be torch.float32, torch.float16, \"int8\" or \"int4\"")
         if emb_dtype == "fp16" and int(m_spa) % 8:
             sys.exit("ERROR: fp16 embedding tables need an embedding dimension divisible by 8")
+        if emb_dtype in ("int8", "int4"):
+            if int(m_spa) % (4 if emb_dtype == "int8" else 8):
+                sys.exit("ERROR: %s row-wise quantized tables need an embedding dimension divisible by %d"
+                         % (emb_dtype, 4 if emb_dtype == "int8" else 8))
+            if emb_host_tables:
+                sys.exit("ERROR: quantized embedding tables are kept in device memory (emb_host_tables is not supported)")
         if qr_flag or md_flag:
             sys.exit("ERROR: --qr-flag / --md-flag embeddings are outside the dlrm_b200 hot path")
         if arch_interaction_op not in ("dot", "cat"):
@@ -162,6 +172,7 @@ class DLRM_Net(nn.Module):
                                  else weighted_pooling)
         self.qr_flag, self.md_flag = False, False
         self.quantize_emb, self.emb_l_q, self.quantize_bits = False, [], 32
+        self._quant_only = emb_dtype in ("int8", "int4")
         ln_emb = np.asarray(ln_emb).astype(np.int64)
         ln_bot = np.asarray(ln_bot).astype(np.int64)
         ln_top = np.asarray(ln_top).astype(np.int64)
@@ -200,6 +211,8 @@ class DLRM_Net(nn.Module):
         if emb_host_cache and not host:
             sys.exit("ERROR: a host row cache (emb_host_cache) needs host embedding tables (emb_host_tables)")
 
+        if self._quant_only and tdist.is_available() and tdist.is_initialized() and tdist.get_world_size() > 1:
+            sys.exit("ERROR: quantized embedding tables are not supported on sharded runs")
         if tdist.is_available() and tdist.is_initialized() and tdist.get_world_size() > 1:
             # one process per GPU (the reference: ext_dist.my_size > 1, dlrm_s_pytorch.py:352-365): tables are
             # placed over the ranks (dlrm_b200/placement.py), the MLPs replicated; max_batch is the GLOBAL batch
@@ -232,6 +245,9 @@ class DLRM_Net(nn.Module):
         if ndevices <= 1:
             self.emb_l, w_list = self.create_emb(m_spa, ln_emb, weighted_pooling)
             self.v_W_l = w_list
+        if self._quant_only:
+            self.quantize_emb, self.quantize_bits = True, self._engine.quant_bits
+            self.emb_l_q = [self._engine.table_q(k) for k in range(self._engine.T)]
         self.bot_l = self.create_mlp(ln_bot, sigmoid_bot)
         self.top_l = self.create_mlp(ln_top, sigmoid_top)
         if loss_function == "mse":
@@ -257,14 +273,37 @@ class DLRM_Net(nn.Module):
         return (1 << 31) + (int(np.max(ln_emb)) * int(m_spa) * 4 if big else 0)
 
     def state_dict(self, *args, **kwargs):
+        if self._engine is not None and self._engine.quant_only:
+            raise RuntimeError("dlrm_b200: this model was built with emb_dtype=%r: its float embedding tables were never "
+                               "stored, so there is no state_dict (emb_l_q[k] holds the packed rows)"
+                               % self._engine.emb_dtype)
         if self._engine is not None and self._engine.host:
             self._engine._host_sync()       # host rows may still be on their way back from the last step
         return super().state_dict(*args, **kwargs)
 
     def load_state_dict(self, state_dict, *args, **kwargs):
-        if self._engine is not None and self._engine.host:
-            self._engine._host_sync()
-        return super().load_state_dict(state_dict, *args, **kwargs)
+        eng = self._engine
+        if eng is not None and eng.quant_only:
+            # the reference's emb_l.{k}.weight (fp32 or fp16, on any device, e.g. an mmap load) is quantized table by
+            # table, QUANT_CHUNK_ROWS rows at a time; the rest loads as usual
+            state_dict = dict(state_dict)
+            for k in range(eng.T):
+                w = state_dict.pop("emb_l.%d.weight" % k, None)
+                if w is None:
+                    if kwargs.get("strict", args[0] if args else True):
+                        raise RuntimeError("dlrm_b200: load_state_dict: missing key emb_l.%d.weight" % k)
+                    continue
+                if tuple(w.shape) != (eng.ln_emb[k], eng.D):
+                    raise RuntimeError("dlrm_b200: load_state_dict: emb_l.%d.weight has shape %s, the model's table is "
+                                       "[%d, %d]" % (k, tuple(w.shape), eng.ln_emb[k], eng.D))
+                eng.quantize_rows(k, w.detach())
+        if eng is not None and eng.host:
+            eng._host_sync()
+        out = super().load_state_dict(state_dict, *args, **kwargs)
+        if eng is not None and self.quantize_emb and not eng.quant_only:
+            for k in range(eng.T):          # quantize_embedding() was called: the packed rows follow the new tables
+                eng.quantize_rows(k, eng.table(k))
+        return out
 
     # ------------------------------------------------------------------ construction
     def create_mlp(self, ln, sigmoid_layer):
@@ -323,8 +362,28 @@ class DLRM_Net(nn.Module):
             return emb_l, v_W_l
         for k in range(ln.size):
             n = int(ln[k])
-            tab = eng.table(k)
             a = float(np.sqrt(1 / n))
+            if eng.quant_only:
+                # the float model's draw for the same seed (same generator, same order), quantized as its
+                # quantize_embedding() would quantize it.  A device draw maps values to elements through the sizes and
+                # strides of its output, so it goes into a whole [n, m] table with the fp32 model's row stride (m: that
+                # model's engine is built with interleave_momentum=False); drawing in chunks would draw other values.
+                # The fp32 temporary is one table (20.5 GB for a 40 M-row MLPerf table), freed before the next.
+                with torch.no_grad():
+                    if big:
+                        W = torch.empty((n, int(m)), dtype=torch.float32, device=eng.device)
+                        assert W.stride() == (int(m), 1)
+                        _uniform_(W, a, gen)
+                    else:
+                        W = torch.from_numpy(np.random.uniform(low=-a, high=a, size=(n, int(m))).astype(np.float32))
+                    eng.quantize_rows(k, W)
+                    del W
+                if weighted_pooling is None:
+                    v_W_l.append(None)
+                elif not eng.learned_row_weights:
+                    v_W_l.append(torch.ones(n, dtype=torch.float32, device=eng.device))
+                continue
+            tab = eng.table(k)
             with torch.no_grad():
                 if big and eng.is_host[k]:
                     # the draw of a device table (same sizes and strides), then copied to host memory
@@ -435,7 +494,23 @@ class DLRM_Net(nn.Module):
         return _DLRMForward.apply(self, sp, torch.is_grad_enabled(), x, *params)
 
     def quantize_embedding(self, bits):
-        sys.exit("ERROR: 4 and 8-bit quantization on GPU is not supported")
+        """dlrm_s_pytorch.py:465-481: pack every table into fbgemm's row-wise `bits`-bit rows (emb_l_q[k], the bytes of
+        torch.ops.quantized.embedding_bag_{byte,4bit}_prepack) and pool from them from now on.  The float tables stay,
+        so state_dict() is unchanged; training is refused afterwards (it would step the float tables while the forward
+        serves the packed ones)."""
+        if bits not in (4, 8):
+            sys.exit("ERROR: quantize_embedding supports 4 and 8 bits (got %r)" % (bits,))
+        if self._dist is not None:
+            sys.exit("ERROR: quantized embedding tables are not supported on sharded runs")
+        eng = self._engine
+        if eng.quant_only:
+            sys.exit("ERROR: the tables are already %d-bit quantized (emb_dtype=%s)" % (eng.quant_bits, eng.emb_dtype))
+        try:
+            eng.quantize_tables(int(bits))
+        except ValueError as e:
+            sys.exit("ERROR: " + str(e))
+        self.emb_l_q = [eng.table_q(k) for k in range(eng.T)]
+        self.quantize_emb, self.quantize_bits = True, int(bits)
 
     # ------------------------------------------------------------------ gradients for torch optimizers
     def _materialise_sparse_grads(self, sp: SparseInput):

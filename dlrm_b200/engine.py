@@ -36,8 +36,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import (ACT_NONE, ACT_RELU, ACT_SIGMOID, DTYPE_F16, DTYPE_F32, GEMM_SIMT_FP32, LOSS_BCE, LOSS_MSE,
-                   LOSS_WBCE, OPT_ADAGRAD, OPT_RWSADAGRAD, OPT_SGD, EmbBwdTable, EmbFwdTable)
+from ._lib import (ACT_NONE, ACT_RELU, ACT_SIGMOID, DTYPE_F16, DTYPE_F32, DTYPE_Q4, DTYPE_Q8, GEMM_SIMT_FP32,
+                   LOSS_BCE, LOSS_MSE, LOSS_WBCE, OPT_ADAGRAD, OPT_RWSADAGRAD, OPT_SGD, EmbBwdTable, EmbFwdTable)
 
 _LOSS = {"mse": LOSS_MSE, "bce": LOSS_BCE, "wbce": LOSS_WBCE}
 _OPT = {"sgd": OPT_SGD, "rwsadagrad": OPT_RWSADAGRAD, "adagrad": OPT_ADAGRAD}
@@ -67,6 +67,17 @@ def round_key(seed: int, step: int, table: int) -> int:
     prefix of (seed, step, table), keyed like the synthetic batches of mlperf.py."""
     base = ((seed * 0xD6E8FEB86659FD93) ^ ((step + 1) * 0x9E3779B97F4A7C15) ^ ((table + 1) * 0x165667B19E3779F9)) & _M64
     return _splitmix64(base)
+
+
+def quant_row_bytes(dim: int, bits: int) -> int:
+    """Bytes of one packed row-wise quantized row (fbgemm's layout): [dim uint8 | fp32 scale | fp32 bias] for 8 bits,
+    [dim/2 bytes | fp16 scale | fp16 bias] for 4 bits."""
+    return dim + 8 if bits == 8 else dim // 2 + 4
+
+
+# Rows quantized per launch when a table is quantized from a float source: a host source (a checkpoint) crosses to the
+# device one chunk at a time, so a load needs one chunk of device memory beyond the packed arena.
+QUANT_CHUNK_ROWS = 1 << 20
 
 
 def fp16_row_stride(dim: int) -> int:
@@ -164,10 +175,17 @@ class Engine:
         dev = self.device
         # ---- table row type.  fp16: rows are stored as IEEE halves, widened to fp32 by the gather and the update, and
         # written back with stochastic rounding keyed by (round_seed, opt_step, global table, global row, column).
-        if emb_dtype not in ("fp32", "fp16"):
-            raise ValueError("emb_dtype must be fp32 or fp16")
+        if emb_dtype not in ("fp32", "fp16", "int8", "int4"):
+            raise ValueError("emb_dtype must be fp32, fp16, int8 or int4")
         self.emb_dtype = emb_dtype
         self.f16 = emb_dtype == "fp16"
+        # Row-wise quantized tables (emb_dtype="int8" / "int4", or quantize_tables() on a float engine): the forward
+        # gathers packed rows from `qtables`; nothing trains them.  quant_only: the float arena was never allocated.
+        self.quant_bits = {"int8": 8, "int4": 4}.get(emb_dtype, 0)
+        self.quant_only = self.quant_bits > 0
+        self.qtables: Optional[torch.Tensor] = None
+        if self.quant_only:
+            self._check_quant_placement(self.quant_bits, host_tables, shards)
         self.round_seed = int(round_seed)
         self.wdtype = torch.float16 if self.f16 else torch.float32
         self.esize = 2 if self.f16 else 4          # bytes per stored table element
@@ -206,8 +224,14 @@ class Engine:
         self.ldw = self.D + self.row_pad if self.interleave else self.D        # row stride in stored elements
         if self.f16:
             self.ldw = fp16_row_stride(self.D)      # D + 8 halves at D % 8 == 0: 272 bytes at D = 128
-        self.tables = torch.zeros((self.dev_rows, self.ldw), dtype=self.wdtype, device=dev)
-        self._head_sep = None if self.interleave else torch.zeros(self.dev_rows, dtype=torch.int32, device=dev)
+        if self.quant_only:
+            self.interleave = False
+            self.tables = self._head_sep = None
+            self.qtables = torch.zeros((self.dev_rows, quant_row_bytes(self.D, self.quant_bits)), dtype=torch.uint8,
+                                       device=dev)
+        else:
+            self.tables = torch.zeros((self.dev_rows, self.ldw), dtype=self.wdtype, device=dev)
+            self._head_sep = None if self.interleave else torch.zeros(self.dev_rows, dtype=torch.int32, device=dev)
         self._host_init()
         self._momentum_sep: Optional[torch.Tensor] = None
         self.acc_ew: Optional[torch.Tensor] = None       # element-wise Adagrad accumulators [total_rows, D]
@@ -681,10 +705,73 @@ class Engine:
     def table(self, k: int) -> torch.Tensor:
         """[rows_k, D] view of table k (strided when the accumulator is interleaved; fp16 with emb_dtype="fp16").
         A host table's view is a CPU tensor of pinned memory, returned after the engine's work has completed."""
+        if self.quant_only:
+            raise RuntimeError("emb_dtype=%s: the engine stores only the packed rows of its tables (table_q(k)); their "
+                               "float rows were never stored" % self.emb_dtype)
         if self.is_host[k]:
             self._host_sync()
             return self._rows_of(self.tables_h, k)[:, :self.D]
         return self._rows_of(self.tables, k)[:, :self.D]
+
+    # ------------------------------------------------------------------ row-wise quantized tables (csrc/quant.cu)
+    def _check_quant_placement(self, bits, host_tables, shards):
+        if bits == 8 and self.D % 4 or bits == 4 and self.D % 8:
+            raise ValueError("%d-bit quantized tables need an embedding dimension divisible by %d (got %d)"
+                             % (bits, 4 if bits == 8 else 8, self.D))
+        if host_tables:
+            raise ValueError("quantized tables are device tables (host_tables is not supported)")
+        if shards is not None and any(int(s["nparts"]) != 1 or int(s["table"]) != k for k, s in enumerate(shards)):
+            raise ValueError("quantized tables are not supported on sharded runs")
+
+    def _refuse_quantized(self, what: str):
+        if self.quant_bits:
+            raise RuntimeError("%s: the embedding tables are %d-bit row-wise quantized, which is inference-only "
+                               "(forward and forward-only graphs)" % (what, self.quant_bits))
+
+    def table_q(self, k: int) -> torch.Tensor:
+        """[rows_k, quant_row_bytes] uint8 view of table k's packed rows: the bytes of
+        torch.ops.quantized.embedding_bag_{byte,4bit}_prepack of its float rows."""
+        if self.qtables is None:
+            raise RuntimeError("the tables are not quantized (emb_dtype=\"int8\"/\"int4\" or quantize_tables())")
+        return self._rows_of(self.qtables, k)
+
+    def quantize_rows(self, k: int, src: torch.Tensor, r0: int = 0):
+        """Quantize float rows src [n, D] (fp32 or fp16, device or host, e.g. an mmap-loaded checkpoint) into rows
+        [r0, r0 + n) of table k's packed rows.  A host source crosses to the device QUANT_CHUNK_ROWS rows at a time;
+        a device source is read in place at its row stride."""
+        if self.qtables is None:
+            raise RuntimeError("the tables are not quantized (emb_dtype=\"int8\"/\"int4\" or quantize_tables())")
+        if src.dim() != 2 or src.shape[1] != self.D or src.dtype not in (torch.float32, torch.float16):
+            raise ValueError("quantize_rows: expected fp32 / fp16 rows of shape [n, %d], got %s %s"
+                             % (self.D, src.dtype, tuple(src.shape)))
+        n = int(src.shape[0])
+        if r0 < 0 or r0 + n > self.ln_emb[k]:
+            raise ValueError("quantize_rows: rows [%d, %d) outside table %d (%d rows)" % (r0, r0 + n, k, self.ln_emb[k]))
+        dst = self.table_q(k)
+        qd = DTYPE_Q8 if self.quant_bits == 8 else DTYPE_Q4
+        with torch.no_grad():
+            for c0 in range(0, n, QUANT_CHUNK_ROWS):
+                part = src[c0:c0 + QUANT_CHUNK_ROWS]
+                if part.device != self.device or part.stride(1) != 1:
+                    part = part.to(self.device).contiguous()
+                _lib.check(self.lib.dlrm_b200_emb_quantize_rows(
+                    part.data_ptr(), DTYPE_F16 if part.dtype == torch.float16 else DTYPE_F32, part.stride(0),
+                    part.shape[0], self.D, dst[r0 + c0:].data_ptr(), qd, dst.stride(0), _stream()), "emb_quantize_rows")
+                self.n_launch += 1
+                del part
+
+    def quantize_tables(self, bits: int):
+        """DLRM_Net.quantize_embedding: pack every (device) float table into `bits`-bit rows; from then on the forward
+        gathers the packed rows and the float tables stay as they are.  Training is refused afterwards."""
+        if bits not in (4, 8):
+            raise ValueError("only 4- and 8-bit row-wise quantization is supported (got %r)" % (bits,))
+        if self.quant_only:
+            raise RuntimeError("the tables are already %d-bit quantized (emb_dtype=%s)" % (self.quant_bits, self.emb_dtype))
+        self._check_quant_placement(bits, self.host, self.shards)
+        self.quant_bits = bits
+        self.qtables = torch.zeros((self.dev_rows, quant_row_bytes(self.D, bits)), dtype=torch.uint8, device=self.device)
+        for k in range(self.T):
+            self.quantize_rows(k, self.table(k))
 
     def _rows_of(self, arena: torch.Tensor, k: int) -> torch.Tensor:
         """Rows of table k in `arena` (a device arena or its host twin; the table decides which)."""
@@ -722,6 +809,7 @@ class Engine:
             raise ValueError("learned weighted pooling is not supported on sharded runs")
 
     def ensure_optimizer_state(self, optimizer: str):
+        self._refuse_quantized("optimizer state")
         if optimizer == "rwsadagrad":
             if not self.interleave and self._momentum_sep is None:
                 self._momentum_sep = torch.zeros(self.dev_rows, dtype=torch.float32, device=self.device)
@@ -829,9 +917,14 @@ class Engine:
         for n, k in enumerate(ks):
             d = arr[n]
             sh = self.shards[k]
-            d.weight = self.tables.data_ptr() + self._abase[k] * self.ldw * self.esize
-            d.ld = self.ldw
-            d.weight_dtype = DTYPE_F16 if self.f16 else DTYPE_F32
+            if self.quant_bits:     # packed rows, ld in bytes
+                d.ld = self.qtables.stride(0)
+                d.weight = self.qtables.data_ptr() + self._abase[k] * d.ld
+                d.weight_dtype = DTYPE_Q8 if self.quant_bits == 8 else DTYPE_Q4
+            else:
+                d.weight = self.tables.data_ptr() + self._abase[k] * self.ldw * self.esize
+                d.ld = self.ldw
+                d.weight_dtype = DTYPE_F16 if self.f16 else DTYPE_F32
             d.indices = sp.indices[k].data_ptr() if sp.indices[k].numel() else 0
             d.offsets = sp.offsets[k].data_ptr()
             d.row_weights = (self.row_weights.data_ptr() + int(self.row_base[k]) * 4
@@ -912,6 +1005,7 @@ class Engine:
         sort-free coalesce) inside the same kernel."""
         chk = _lib.check
         if link:
+            self._refuse_quantized("training gather")
             total = sp.nnz_total if sp.include_last else sum(int(i.numel()) for i in sp.indices)
             self._ensure_link(total)
         # host tables: stage the rows first (unless emb_link already staged this batch for its update)
@@ -1081,6 +1175,7 @@ class Engine:
     def emb_link(self, sp: SparseInput):
         """Thread this batch's (table,row) occurrences onto per-row lists.  Indices only: may be
         issued on a side stream, concurrently with the forward pass."""
+        self._refuse_quantized("emb_link")
         total = sp.nnz_total if sp.include_last else sum(int(i.numel()) for i in sp.indices)
         self._ensure_link(total)
         if self.host and self._staged is not sp:
@@ -1107,6 +1202,7 @@ class Engine:
         """Fused embedding backward + sparse optimizer for every local shard (coalesce + row update in place).
         dY is None: the gradient rows are where `route_dy` says (dT, or the receive slabs of a sharded run);
         explicit dY: dY[b, k, :] with the given strides.  Tiny tables go through the dense two-pass kernels."""
+        self._refuse_quantized("emb_update")
         routed = dY is None
         dy_off = self.route_dy if routed else [k * stride_table for k in range(self.T)]
         ss = self.dy_stride if routed else stride_sample
@@ -1223,6 +1319,7 @@ class Engine:
         """Everything between the loss and the parameter gradients.  Leaves dense grads in
         dense_grad and the per-bag embedding grads in dT[:, 1:, :].  update=(optimizer, clr) also
         applies the fused embedding update (on a side stream on the tensor-core path)."""
+        self._refuse_quantized("backward")
         B = X.shape[0]
         FD = self.F * self.D
         if self.tc:
@@ -1279,6 +1376,7 @@ class Engine:
     def backward_from_output_grad(self, X: torch.Tensor, sp: SparseInput, gp: torch.Tensor):
         """Backward pass started from dE/dp computed OUTSIDE (autograd of the module's output).
         Leaves dense grads in dense_grad (slabs) and per-bag embedding grads in dT[:, 1:, :]."""
+        self._refuse_quantized("backward")
         B = X.shape[0]
         nt = len(self.ln_top) - 1
         p = self.top_act[nt - 1]
@@ -1348,6 +1446,7 @@ class Engine:
         overlaps the bottom MLP of step i+1 (the dense optimizer does not depend on it).  The caller
         must then use a different batch buffer for the next step and call `sync_update()` before
         reading the tables from another stream."""
+        self._refuse_quantized("train_step")
         self.ensure_optimizer_state(optimizer)
         self._join_update = bool(join_update) or not self.tc
         try:
@@ -1837,7 +1936,8 @@ class GraphedTrainStep:
         self.target = target if target is not None else stage.target
         self.B = self.X.shape[0]
         self.lr, self.optimizer, self.device_lr = lr, optimizer, bool(device_lr)
-        eng.ensure_optimizer_state(optimizer)
+        if train or not eng.quant_bits:
+            eng.ensure_optimizer_state(optimizer)
         if self.device_lr and eng.lr_scalar is None:
             eng.lr_scalar = torch.zeros(1, dtype=torch.float32, device=eng.device)
         if warmup > 0:

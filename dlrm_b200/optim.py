@@ -40,8 +40,8 @@ class _Fused(torch.optim.Optimizer):
         if net is None:
             raise NotEngineParameters("dlrm_b200.optim optimizers take the parameters of a dlrm_b200.DLRM_Net")
         self.net = net() if callable(net) else net
+        self.net._engine.ensure_optimizer_state(self._name)    # refuses quantized (inference-only) tables
         self.net._fused_opt = self
-        self.net._engine.ensure_optimizer_state(self._name)
 
     def zero_grad(self, set_to_none: bool = True):
         self.net._pending = None      # discards a backward() whose step() was skipped

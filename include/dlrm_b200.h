@@ -48,8 +48,11 @@ enum { DLRM_LOSS_MSE = 0, DLRM_LOSS_BCE = 1, DLRM_LOSS_WBCE = 2 };
 enum { DLRM_OPT_SGD = 0, DLRM_OPT_RWSADAGRAD = 1, DLRM_OPT_ADAGRAD = 2 };
 /* GEMM back ends */
 enum { DLRM_GEMM_SIMT_FP32 = 0, DLRM_GEMM_TC_BF16X3 = 1, DLRM_GEMM_TC_BF16 = 2 };
-/* storage type of embedding table rows (weight_dtype of the table descriptors) */
-enum { DLRM_DTYPE_F32 = 0, DLRM_DTYPE_F16 = 1 };
+/* storage type of embedding table rows (weight_dtype of the table descriptors).  The row-wise quantized types are
+ * fbgemm's packed rows (torch.ops.quantized.embedding_bag_{byte,4bit}_prepack), forward-only, `ld` in bytes:
+ *   DLRM_DTYPE_Q8: [dim uint8 | fp32 scale | fp32 bias], dim % 4 == 0, 4-byte aligned rows;
+ *   DLRM_DTYPE_Q4: [dim/2 bytes, column 2j in the low nibble of byte j | fp16 scale | fp16 bias], dim % 8 == 0. */
+enum { DLRM_DTYPE_F32 = 0, DLRM_DTYPE_F16 = 1, DLRM_DTYPE_Q8 = 2, DLRM_DTYPE_Q4 = 3 };
 
 int dlrm_b200_abi_version(void);
 const char* dlrm_b200_last_error(void);
@@ -89,13 +92,29 @@ typedef struct {
   int64_t out_off, out_stride;
   int64_t row_lo, row_n;
   int32_t weight_dtype;     /* DLRM_DTYPE_F32 (0) or DLRM_DTYPE_F16: fp16 rows are widened to fp32 and summed as above,
-                             * so the pooled output equals the fp32 gather over the widened table bit for bit */
+                             * so the pooled output equals the fp32 gather over the widened table bit for bit.
+                             * DLRM_DTYPE_Q8 / Q4 (dlrm_b200_emb_bag_fwd only; whole tables, no row range): every
+                             * occurrence j of row r adds, column by column and in index order,
+                             *   acc = fmaf(s, q, acc + b),  s = scale_r * w_j,  b = bias_r * w_j  (both rounded to fp32)
+                             * with w_j = row_weights[r] (1 without them) and the fp16 scale / bias of Q4 widened first:
+                             * bit-identical to torch.ops.quantized.embedding_bag_{byte,4bit}_rowwise_offsets on the
+                             * CPU.  ld = 0 means the packed width (dim + 8 or dim/2 + 4 bytes). */
 } dlrm_emb_fwd_table_t;
 
 int dlrm_b200_emb_bag_fwd(const dlrm_emb_fwd_table_t* tables /*[host]*/, int num_tables, int dim,
                           int64_t batch, int idx_bytes, int include_last,
                           float* out, int64_t out_stride_sample, int64_t out_stride_table,
                           void* stream);
+
+/* Row-wise quantization of `rows` float rows (src_dtype DLRM_DTYPE_F32 or F16, row stride ld_src in elements, so
+ * the engine's interleaved rows work as they are) into packed rows of dst_dtype DLRM_DTYPE_Q8 / Q4 (row stride
+ * ld_dst bytes, 0 = the packed width).  Byte-identical to torch.ops.quantized.embedding_bag_{byte,4bit}_prepack of
+ * the same (widened) values for finite rows; a caller quantizes a table in chunks by offsetting both pointers.
+ *   Q8: bias = min, scale = (max - min) / 255, q = rint((x - min) * (255 / ((max - min) + 1e-8))).
+ *   Q4: bias = fp16(min), scale = fp16((max - bias) / 15) (1 when the range or that is 0, or 1 / scale is inf),
+ *       q = clamp(rint((x - bias) * (1 / scale)), 0, 15). */
+int dlrm_b200_emb_quantize_rows(const void* src, int src_dtype, int64_t ld_src, int64_t rows, int dim, void* dst,
+                                int dst_dtype, int64_t ld_dst, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Embedding backward fused with the sparse optimizer
